@@ -1,4 +1,4 @@
-"""garecon — B200-native batch reconcile-diff engine for the aws-global-accelerator-controller hot path.
+"""garecon — H100-native batch reconcile-diff engine for the aws-global-accelerator-controller hot path.
 
 The directory name carries the upstream project's hyphens, so import it with
 `importlib.import_module("aws-global-accelerator-controller_b200")` (tests/conftest.py does this and

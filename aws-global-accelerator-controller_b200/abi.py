@@ -1,7 +1,7 @@
 """ctypes mirror of include/garecon.h and the loader for libgarecon.so.
 
 This is host plumbing over the C ABI (the drop-in boundary): the structs below are field-for-field the
-ones in include/garecon.h.  There is no CPU fallback: if the CUDA library is missing or no sm_100 device
+ones in include/garecon.h.  There is no CPU fallback: if the CUDA library is missing or no sm_90 device
 is present, `Engine()` raises.
 """
 from __future__ import annotations

@@ -1,7 +1,7 @@
 // gar_common.h — types and byte-level primitives shared by every kernel of the diff engine.
 //
 // All row logic is written as GAR_HD functions so that the very same code can be compiled (a) by nvcc into the
-// sm_100a kernels that ship in libgarecon.so and (b) by g++ into tests/hostsim, a debugging build that lets
+// sm_90a kernels that ship in libgarecon.so and (b) by g++ into tests/hostsim, a debugging build that lets
 // the CPU-only CI run the device logic against the oracle.  (b) is a test artefact; the product has no CPU path.
 #pragma once
 

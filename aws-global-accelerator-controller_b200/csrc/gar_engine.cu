@@ -1,10 +1,10 @@
-// gar_engine.cu — CUDA backend (sm_100a) and C ABI of the reconcile-diff engine.
+// gar_engine.cu — CUDA backend (sm_90a) and C ABI of the reconcile-diff engine.
 //
 // Implements include/garecon.h.  Stage logic lives in gar_rows.h / gar_pipeline.h; this file supplies what
 // is specific to the GPU: kernels for the data-parallel stages, the device-wide exclusive scan, the stable LSD
 // radix sort that orders hash-index buckets, device/pinned memory management, stream + event timing.
 //
-// There is deliberately no CPU path in this library: every entry point needs a live sm_100 device.
+// There is deliberately no CPU path in this library: every entry point needs a live sm_90 (H100) device.
 
 #include <cuda_runtime.h>
 #include <unistd.h>
@@ -25,7 +25,7 @@
 #include "gar_pipeline.h"
 #include "gar_shard.h"
 
-#define GAR_VERSION_STRING "garecon 0.1.0 (sm_100a)"
+#define GAR_VERSION_STRING "garecon 0.1.0 (sm_90a)"
 
 // ------------------------------------------------------------------ kernels
 
@@ -455,7 +455,7 @@ static std::string g_create_error = "";
 // Sharded-mode pack, shared-memory variant (gar_shard.h FShPackRows; optional, GAR_PACK_TMA=1): one thread per selected row.  The
 // 256 rows of a block own one contiguous byte range of their destination's slab, so the block assembles it in shared memory and
 // one thread writes it with a bulk store (cp.async.bulk.global.shared::cta).  Blocks that straddle two destinations or exceed
-// the tile store directly.  Kept for the record: it lost against plain per-thread stores both locally and over NVLink.
+// the tile store directly.  Off by default: plain per-thread stores are the default path.
 constexpr u32 PACK_TILE = 40 * 1024;
 __device__ __forceinline__ void bulk_s2g(void *dst, const void *src, u32 bytes) {
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(smem_addr(src)), "r"(bytes) : "memory");
@@ -500,8 +500,7 @@ __global__ void __launch_bounds__(256) k_shard_pack_rows(const __grid_constant__
 
 // Peer push (sharded mode, gar_shard_pack_peers): finished level groups of the staged blobs go to the other GPUs' receive arenas
 // over NVLink as 16-byte coalesced stores, one grid row per destination.  Runs on a high-priority stream beside the pack
-// kernels of the later levels.  (Measured at 8 GPUs, 2.6 GB to 7 peers per rank: copy engines 340 GB/s aggregate, last byte at
-// 7.8 ms; this kernel: last byte 0.2 ms after the last pack kernel, at 6.8 ms; NCCL all-to-all after a separate pack: 7.9 ms.)
+// kernels of the later levels.
 struct PushDesc {
   const uint4 *src[GAR_SHARD_MAX_RANKS];
   uint4 *dst[GAR_SHARD_MAX_RANKS];
@@ -657,8 +656,7 @@ struct gar_engine {
 
   // ---- Backend interface (gar_pipeline.h)
   // GAR_PACK_TMA=1: the sharded pack assembles each block's slab range in shared memory and bulk-stores it (k_shard_pack_rows).
-  // Measured on the B200 (profiles/r02_pack_tma_ab.json): 10 % slower than per-thread stores into local memory (5.54 vs 5.02 ms,
-  // 2*10^6 objects) and 2.4x slower straight into peer arenas over NVLink (16.6 vs 6.8 ms per round-1 pack at 8 GPUs) — off.
+  // Off by default (per-thread stores).
   bool pack_tma = false;
   template <class F>
   void for_each(const char *name, u32 n, const F &f) {
@@ -737,7 +735,7 @@ struct gar_engine {
     CK(cudaGraphLaunch(graph_exec, stream));
   }
   // environment GAR_NO_TMA=1: every staged row pass in its direct-load form; GAR_TMA_ALL=1: every one staged (A/B measurements).
-  // Default: each pass in the form that measured faster on the B200 (F::kStageByDefault).
+  // Default: each pass in the form that measured faster on the H100 (F::kStageByDefault).
   bool staged_passes = true, staged_all = false;
   template <class F>
   void for_each_staged(const char *name, u32 n, const F &f) {
@@ -788,7 +786,7 @@ struct gar_engine {
       return;
     }
     size_t blocks = (n + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;  // 16 blocks per SM of an H100 SXM
     k_fill32<<<(unsigned)blocks, 256, 0, stream>>>(p, v, n);
     launches++;
   }
@@ -1284,8 +1282,8 @@ int gar_engine_create(const gar_config *cfg, gar_engine **out) {
     return GAR_E_NO_DEVICE;
   }
   cudaDeviceProp prop;
-  if (cudaGetDeviceProperties(&prop, cfg->device) != cudaSuccess || prop.major != 10) {
-    g_create_error = "device is not sm_100 (this library ships sm_100a code only)";
+  if (cudaGetDeviceProperties(&prop, cfg->device) != cudaSuccess || prop.major != 9 || prop.minor != 0) {
+    g_create_error = "device is not sm_90 (this library ships sm_90a code only)";
     cudaGetLastError();
     return GAR_E_NO_DEVICE;
   }

@@ -1,6 +1,6 @@
 // gar_pipeline.h — the diff as a sequence of data-parallel stages over a Backend.
 //
-// Backend = how a stage runs: the CUDA backend (gar_engine.cu) launches sm_100a kernels on a stream; the
+// Backend = how a stage runs: the CUDA backend (gar_engine.cu) launches sm_90a kernels on a stream; the
 // host-simulation backend (tests/hostsim) runs the same functors in loops so the CPU-only test tier can
 // exercise the device logic.  Stages, functors and their order live here once.
 //
@@ -79,7 +79,7 @@ struct FTokenise {
   Work W;
   static constexpr int kStageCols = 1;
   static constexpr u32 kStageBytes = 24 * 1024;  // 256 lbIngress hostnames of ~70 bytes
-  static constexpr bool kStageByDefault = true;
+  static constexpr bool kStageByDefault = true;  // H100 SXM: 0.146 ms staged vs 0.149 ms direct
   GAR_HD void operator()(u32 i) const { tokenise_hostname(T, W, i); }
   GAR_HD const u8 *stage_slab(int) const { return T.o.slab; }
   GAR_HD bool stage_window(int, u32 r0, u32 r1, u64 *lo, u64 *hi) const {
@@ -127,7 +127,7 @@ struct FPrepareRecord {
   u32 *big, *huge;  // [0] = count, then record rows
   static constexpr int kStageCols = 2;  // window 0: record names, window 1: the records' values
   static constexpr u32 kStageBytes = 16 * 1024;  // 256 names of ~28 bytes; ~130 values of ~95 bytes
-  static constexpr bool kStageByDefault = false;  // measured on the B200 (profiles/r02_tma_ab.json): 0.297 ms staged vs 0.265 ms direct
+  static constexpr bool kStageByDefault = true;  // H100 SXM: 0.418 ms staged vs 0.430 ms direct (bench.py, 10^6 objects)
   GAR_HD const u8 *stage_slab(int) const { return T.a.slab; }
   GAR_HD bool stage_window(int c, u32 r0, u32 r1, u64 *lo, u64 *hi) const {
     if (c == 0) {
@@ -176,7 +176,7 @@ struct FPrepareRecord {
 };
 // fixed grid of BIG_BLOCKS x 256 threads: block b takes big records b, b + BIG_BLOCKS, ... and its threads stride over the
 // values; the (few) huge records are strided over by the whole grid
-constexpr u32 BIG_BLOCKS = 592;  // 4 x 148 SMs
+constexpr u32 BIG_BLOCKS = 528;  // 4 x 132 SMs (H100 SXM)
 struct FClassifyBigRecords {
   DevTables T;
   Work W;

@@ -1,7 +1,7 @@
 // gar_rows.h — per-row decision logic of the diff engine (one call = one table row).
 //
 // Each function states the reference code it stands for (paths relative to the reference root).
-// Everything here is GAR_HD: nvcc compiles it into the sm_100a kernels of libgarecon.so; tests/hostsim
+// Everything here is GAR_HD: nvcc compiles it into the sm_90a kernels of libgarecon.so; tests/hostsim
 // compiles the same text with g++ for CPU-side debugging of the device logic.
 #pragma once
 

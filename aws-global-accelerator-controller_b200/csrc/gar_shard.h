@@ -1,5 +1,5 @@
 // gar_shard.h — ONE cluster sharded by key hash across ranks (SURVEY.md §8 row e, BASELINE configs[3]:
-// "10^7 objects sharded by key-hash across 8xB200 with one NCCL all-to-all").
+// "10^7 objects sharded by key-hash across GPUs with one NCCL all-to-all").
 //
 // Every rank starts with an arbitrary contiguous slice of each list (the packer just cuts the lister output and the
 // paginated AWS lists into n_ranks ranges; include/garecon.h "sharded mode").  The diff is a join DAG over several keys,
@@ -446,7 +446,7 @@ struct FShPackRows {
 };
 // The rest of the cut strings: a fixed number of workers stride over the rows, SH_COPY_LANES lanes per row.  Leaves at once when
 // no string was cut (the flag stays on the device: no host round-trip decides about this launch).
-constexpr u32 SH_COPY_LANES = 8, SH_LONG_WORKERS = 148 * 8 * 256;
+constexpr u32 SH_COPY_LANES = 8, SH_LONG_WORKERS = 132 * 8 * 256;  // 8 blocks on each of the 132 SMs of an H100 SXM
 struct FShPackLong {
   LevelSrc src;
   int n_str;

@@ -8,7 +8,7 @@ One "step" = one complete diff (both controllers, every object, orphans) over on
 
 Workload (config.workload): BASELINE.json configs[2] — 10^6 Service+Ingress, every object carrying a
 multi-hostname route53 annotation, ~10^6 accelerators / 2*10^6 record sets on the AWS side (the config the
-metric "objects reconciled/sec at 10^6" is quoted on; it fits one B200).  N > 1 is weak scaling: every rank
+metric "objects reconciled/sec at 10^6" is quoted on; it fits one H100).  N > 1 is weak scaling: every rank
 diffs its own 10^6-object cluster (independent clusters shard with no data-path collective; DESIGN.md §Multi-GPU).
 
 JSON keys beyond the base contract:
@@ -18,6 +18,9 @@ JSON keys beyond the base contract:
              every table + kernels + D2H of the whole change set inside the timed region
   roofline   HBM roofline of the dominant kernel and of the whole pipeline (CUDA events on the engine's stream)
   cpu_baseline  the oracle (C++ port of the reference decision functions, indexed, all host threads) on a bounded sample
+  device     name and power limit of the GPU the numbers were measured on
+
+--dump-outputs DIR writes the change set of the last timed step as DIR/<name>.npy (float64; see dump_outputs).
 The Go reference itself is NOT timed: there is no Go toolchain in this image (BASELINE.md §2).
 """
 from __future__ import annotations
@@ -36,23 +39,106 @@ from pathlib import Path
 
 REPO = Path(__file__).resolve().parent
 sys.path.insert(0, str(REPO))
+sys.dont_write_bytecode = True  # the tree may be read-only; bench.py writes nothing into it
 
 METRIC = "objects reconciled/sec at 10^6 Service+Ingress; change-set bit-exact vs Go ref"
 UNIT = "objects/s"
 
 
 def _peaks():
-    p = REPO / "MEASURED_PEAKS.json"
-    if p.exists():
-        try:
-            return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-        except Exception:
-            pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    """HBM bandwidth the roofline fractions are taken against: the data-sheet figure (a denominator, not a measured rate)."""
+    return 3350.0, "NVIDIA H100 SXM data sheet: 3.35 TB/s HBM3"
+
+
+def _device_info(idx: int) -> dict:
+    """Name and power limit of the GPU: an absolute number in the line is only meaningful beside them."""
+    info = {"name": None, "power_limit_w": None}
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits", "-i", str(idx)],
+                             capture_output=True, text=True, timeout=30).stdout.strip().split(",")
+        info["name"] = out[0].strip()
+        info["power_limit_w"] = float(out[1])
+    except Exception:
+        pass
+    if info["name"] is None:
+        import torch
+        info["name"] = torch.cuda.get_device_name(idx)
+    return info
+
+
+def _require_built():
+    """bench.py runs on the tree as __graft_entry__.build() left it and never compiles (the tree may be read-only)."""
+    import __graft_entry__ as ge
+    libs = (ge.PKG / "libgarecon.so", ge.PKG / "synth" / "libgarecon_synth.so", REPO / "oracle" / "liboracle.so")
+    missing = [str(p.relative_to(REPO)) for p in libs if not p.exists()]
+    if missing:
+        raise SystemExit(f"bench.py: {', '.join(missing)} not built; run `python __graft_entry__.py` first")
+
+
+DUMP_ROWS = 1 << 17  # rows per dumped array: a longer array is dumped as a fixed, seeded sample of this many rows
+DUMP_SEED = 20240601
+
+
+def _device_bytes(torch, ptr, nbytes: int):
+    """Host copy (numpy uint8) of `nbytes` of device memory at `ptr` (an engine-owned buffer on the current device)."""
+    import numpy as np
+    if not nbytes:
+        return np.zeros(0, dtype=np.uint8)
+
+    class _Dev:
+        __cuda_array_interface__ = {"shape": (int(nbytes),), "typestr": "|u1", "data": (int(ptr), False), "version": 3}
+    return torch.as_tensor(_Dev(), device="cuda").cpu().numpy()
+
+
+def dump_outputs(torch, abi, cs, out_dir: Path) -> dict:
+    """Write the change set a gar_diff_device call left on the device (`cs`: device pointers, valid until the next diff or load)
+    as float64 .npy files, so that two builds can be compared output for output on the same seeded workload:
+      status_ga, status_r53, derived [n]; ops [n_ops, 6] (head obj sub a0 a1 a2); section_begin [5]; tok_code [n_lbi];
+      tok_name, tok_region [n_lbi, 2] (slab offset, length); dport_begin [n + 1]; dports [n_dports]
+    An array longer than DUMP_ROWS rows is replaced by a sample of DUMP_ROWS rows drawn with a fixed seed (same for every array
+    of that length), written with its row indices as <name>_rows.npy.  checksums.npy holds the CRC-32 of every complete array
+    (abi.ChangeSet.ARRAYS order), so rows outside the sample are compared too.  Returns {file: shape}."""
+    import zlib
+    import numpy as np
+    P = lambda p: C.cast(p, C.c_void_p).value
+    n, n_ops, n_lbi, n_dp = int(cs.n_objects), int(cs.n_ops), int(cs.n_lbi), int(cs.n_dports)
+    full = {
+        "status_ga": _device_bytes(torch, P(cs.status_ga), 4 * n).view(np.uint32),
+        "status_r53": _device_bytes(torch, P(cs.status_r53), 4 * n).view(np.uint32),
+        "derived": _device_bytes(torch, P(cs.derived), 4 * n).view(np.uint32),
+        "ops": _device_bytes(torch, P(cs.ops), 24 * n_ops).view(abi.OP_DTYPE),
+        "section_begin": np.array(list(cs.section_begin), dtype=np.uint64),
+        "tok_code": _device_bytes(torch, P(cs.tok_code), n_lbi),
+        "tok_name": _device_bytes(torch, P(cs.tok_name), 8 * n_lbi).view(np.uint64),
+        "tok_region": _device_bytes(torch, P(cs.tok_region), 8 * n_lbi).view(np.uint64),
+        "dport_begin": _device_bytes(torch, P(cs.dport_begin), 4 * (n + 1)).view(np.uint32),
+        "dports": _device_bytes(torch, P(cs.dports), 4 * n_dp).view(np.int32),
+    }
+    out_dir.mkdir(parents=True, exist_ok=True)
+    written = {}
+
+    def save(name, arr):
+        np.save(out_dir / f"{name}.npy", arr)
+        written[f"{name}.npy"] = list(arr.shape)
+
+    save("checksums", np.array([zlib.crc32(np.ascontiguousarray(full[k]).view(np.uint8).tobytes()) for k in abi.ChangeSet.ARRAYS], dtype=np.float64))
+    for name, a in full.items():
+        if len(a) > DUMP_ROWS:
+            rows = np.sort(np.random.default_rng([DUMP_SEED, len(a)]).choice(len(a), DUMP_ROWS, replace=False))
+            a = a[rows]
+            save(f"{name}_rows", rows.astype(np.float64))
+        if a.dtype == abi.OP_DTYPE:
+            a = np.stack([a[f].astype(np.float64) for f in abi.OP_DTYPE.names], axis=1)
+        elif name in ("tok_name", "tok_region"):
+            a = np.stack([(a & np.uint64(abi.OFF_MASK)).astype(np.float64), (a >> np.uint64(abi.OFF_BITS)).astype(np.float64)], axis=1)
+        else:
+            a = a.astype(np.float64)
+        save(name, a)
+    return written
 
 
 class ClockSampler:
-    """nvidia-smi sampling during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampling during the timed region (SM clock, power draw, throttle reasons)."""
 
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -259,9 +345,7 @@ def run_reference(args, rank, world):
     as the GPU arm: the full --objects cluster of --config, same generator seed and slab layout."""
     if rank != 0:
         return
-    import __graft_entry__ as ge
-    ge.build_synth()
-    ge.build_oracle()
+    _require_built()
     synth = importlib.import_module("aws-global-accelerator-controller_b200.synth")
     ob = importlib.import_module("oracle.binding")
     cores = os.cpu_count() or 1
@@ -307,11 +391,14 @@ def _workload_name(config, objects):
     return f"BASELINE configs[{config - 1}]: {objects} objects, {_WORKLOADS.get(config, '')}"
 
 
+L2_BYTES = 50e6  # H100 SXM
+
+
 def _cache_note(bytes_per_gpu):
-    """how the timed iterations avoid a warm L2 (126 MB): inputs larger than L2, or say that they are not"""
-    if bytes_per_gpu > 2 * 126e6:
-        return f"inputs ({bytes_per_gpu / 1e6:.0f} MB per GPU) larger than L2 (126 MB); no flush needed"
-    return f"inputs ({bytes_per_gpu / 1e6:.0f} MB per GPU) do NOT exceed L2 (126 MB): an L2-sized scratch buffer is rewritten between timed steps"
+    """how the timed iterations avoid a warm L2 (50 MB): inputs larger than L2, or say that they are not"""
+    if bytes_per_gpu > 2 * L2_BYTES:
+        return f"inputs ({bytes_per_gpu / 1e6:.0f} MB per GPU) larger than L2 (50 MB); no flush needed"
+    return f"inputs ({bytes_per_gpu / 1e6:.0f} MB per GPU) do NOT exceed L2 (50 MB): a scratch buffer larger than L2 is rewritten between timed steps"
 
 
 SHARD_CHUNKS = 16  # the sharded cluster is always generated as 16 chunks, whatever the number of GPUs
@@ -489,7 +576,7 @@ def sharded_measure(args, R, rank, world, local_rank, n_total, cfg_id, steps, wa
         "gpu_launches": launches, "clocks": clocks,
         "bytes_sent": {"per_rank": [c[2] for c in allc], "max": sent_max,
                        "nvlink_gbs_per_direction_in_transfer": round(sent_max / max(sum(ph_max.get(k, 0) for k in xfer), 1e-9) / 1e6, 1),
-                       "transfer_phases": xfer, "nvlink_peak_gbs_per_direction": 900.0, "nvlink_measured_peer_copy_gbs": 770.0},
+                       "transfer_phases": xfer, "nvlink_peak_gbs_per_direction": 450.0},
         "roofline": {"bound": "hbm", "kernel": "whole sharded step (route, pack, exchange, merge, diff)", "achieved": achieved, "peak": peak * world,
                      "unit": "GB/s", "frac": achieved / (peak * world), "traffic": None, "peak_source": peak_src + f" x {world} GPUs"},
         "phases_ms_rank0": {k: round(v, 3) for k, v in phases.items()},
@@ -512,7 +599,6 @@ def run_sharded(args, rank, world, local_rank):
     """`--mode sharded`: the sharded step as the bench line's own metric (the default invocation under torchrun reports it as
     the `sharded` record of the replicas line instead)."""
     import torch
-    import __graft_entry__ as ge
     ranks_mod = importlib.import_module("aws-global-accelerator-controller_b200.ranks")
     dev = torch.device("cuda", local_rank)
     R = ranks_mod.Ranks(backend="nccl", device=dev)
@@ -522,7 +608,7 @@ def run_sharded(args, rank, world, local_rank):
         R.dist.init_process_group("nccl", rank=0, world_size=1, device_id=dev)
         R.owns_group = True
     if rank == 0:
-        ge.ensure_built()
+        _require_built()
     R.barrier()
     cfg_id = 4 if args.config == 3 else args.config  # default workload of this mode: configs[3] = generator preset 4
     rec = sharded_measure(args, R, rank, world, local_rank, args.objects, cfg_id, args.steps, args.warmup, with_single=not args.no_single)
@@ -558,7 +644,11 @@ def main():
                     help="sharded mode data path: p2p = pack kernels store straight into the other GPUs' receive arenas (CUDA IPC peer memory); "
                          "nccl = pack into a send buffer, torch.distributed all_to_all_single, unpack")
     ap.add_argument("--no-single", action="store_true", help="sharded: skip the single-GPU run of the same cluster (no checksum comparison)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="replicas, rank 0: write the change set of the last timed step as DIR/<name>.npy (float64, sampled rows + checksums)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3) if args.impl == "garecon" else args.warmup
 
     rank = int(os.environ.get("RANK", "0"))
@@ -575,7 +665,6 @@ def main():
     if args.mode == "sharded":
         run_sharded(args, rank, world, local_rank)
         return
-    import __graft_entry__ as ge
     pkg = importlib.import_module("aws-global-accelerator-controller_b200")
     synth = importlib.import_module("aws-global-accelerator-controller_b200.synth")
     ranks_mod = importlib.import_module("aws-global-accelerator-controller_b200.ranks")
@@ -583,7 +672,7 @@ def main():
     numa = binding.node
     R = ranks_mod.Ranks(backend="nccl", device=torch.device("cuda", local_rank))
     if rank == 0:
-        ge.ensure_built()
+        _require_built()
     R.barrier()
     abi = pkg.abi
     barrier, max_over_ranks = R.barrier, R.max_over_ranks
@@ -598,7 +687,7 @@ def main():
     pinned_bytes, pinned_addrs = _pin_host_tables(torch, abi, o, a)
     binding.release()
     # inputs that fit in L2 would make every timed step after the first an L2-warm re-read: rewrite an L2-sized buffer between steps
-    flush = h2d_bytes <= 2 * 126e6
+    flush = h2d_bytes <= 2 * L2_BYTES
     flush_buf = torch.empty(256 << 20, dtype=torch.uint8, device=f"cuda:{local_rank}") if flush else None
 
     # reprepare=True: every timed step runs the COMPLETE pipeline (digests, indexes, decide, placement); without it the
@@ -628,6 +717,7 @@ def main():
     barrier()
     t1 = time.perf_counter()
     dt_dev = max_over_ranks(t1 - t0 - t_flush)
+    dumped = dump_outputs(torch, abi, cs, Path(args.dump_outputs)) if args.dump_outputs and rank == 0 else None
     b_alg = eng.algorithmic_bytes(cs)
     n_ops = int(cs.n_ops)
     n_pairs = eng.counters().get("r53_pairs", 0)
@@ -706,7 +796,7 @@ def main():
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": dt_dev / args.steps * 1e3, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-            "dtype": "u8/u32 (bytes and indices)", "data": "synthetic",
+            "dtype": "u8/u32 (bytes and indices)", "data": "synthetic", "device": _device_info(local_rank),
             "config": {"workload": _workload_name(args.config, args.objects) + f" per GPU; {a.n_accels} accelerators, {a.n_records} record sets, {a.n_lbs} load balancers",
                        "slab_layout": args.layout, "objects_per_gpu": args.objects, "parallelism": f"replicas x{world} (independent clusters, no collective)",
                        "cache": _cache_note(h2d_bytes), "seed": int(cfg.seed),
@@ -723,16 +813,12 @@ def main():
                          "stages_ms": {s[0]: round(s[1], 4) for s in stages}},
             "kernel_ms_per_step_cuda_events": ms_kernels / args.steps,
         }
+        if dumped is not None:
+            line["dumped_outputs"] = {"dir": str(args.dump_outputs), "files": dumped}
         # the dominant kernel's own byte model (DESIGN.md "Per-kernel byte model"); the pipeline figure is the headline
         frac_ga = float(((hcs.status_ga & 0xFF) > 2).sum() + ((hcs.status_ga & 0xFF) == 1).sum()) / max(args.objects, 1)
         sb = [int(x) for x in hcs.section_begin]
         models = kernel_byte_models(o, a, sb[1] - sb[0], n_pairs, frac_ga)
-        traffic, traffic_src = {}, None
-        for tp in (REPO / "profiles" / "r02_ncu_traffic.json", REPO / "profiles" / "r01_ncu_traffic.json"):
-            if tp.exists() and args.config == 3 and args.objects == 1_000_000:  # the capture is of this exact workload
-                traffic = json.loads(tp.read_text()).get("dram_bytes_per_launch", {})
-                traffic_src = f"profiles/{tp.name} (ncu --set full, same workload)"
-                break
         # every stage with a byte model: its own achieved GB/s and fraction of the HBM roofline (CUDA-event stage times)
         line["roofline"]["kernels"] = {name: {"ms": round(ms, 4), "bytes": models[name], "achieved_gbs": round(models[name] / (ms * 1e-3) / 1e9, 1),
                                               "frac": round(models[name] / (ms * 1e-3) / 1e9 / peak, 4)}
@@ -742,8 +828,6 @@ def main():
             line["roofline"]["achieved"] = kb / (top[1] * 1e-3) / 1e9
             line["roofline"]["frac"] = line["roofline"]["achieved"] / peak
             line["roofline"]["kernel_bytes"] = kb
-            line["roofline"]["traffic"] = traffic.get(top[0])
-            line["roofline"]["traffic_source"] = traffic_src if top[0] in traffic else None
         else:
             line["roofline"]["achieved"] = pipe_achieved
             line["roofline"]["frac"] = pipe_achieved / peak

@@ -1,5 +1,5 @@
 /*
- * garecon.h — C ABI of the B200 batch reconcile-diff engine (libgarecon.so).
+ * garecon.h — C ABI of the H100 batch reconcile-diff engine (libgarecon.so).
  *
  * Drop-in boundary for ONE path of h3poteto/aws-global-accelerator-controller: the
  * desired-vs-actual decision logic that the Go controller runs per work item behind
@@ -24,7 +24,7 @@
  * Ownership: the caller owns every input buffer and may free it as soon as gar_snapshot_load returns
  * (cgo must not let C retain Go pointers); the engine owns a change set until gar_changeset_free.
  * Errors: every call returns GAR_OK or a negative gar_rc; gar_last_error gives the text.  The engine
- * never aborts and has no CPU fallback: without a usable sm_100 device every call fails.
+ * never aborts and has no CPU fallback: without a usable sm_90 device every call fails.
  * Threading: calls on one engine are serialised by an internal mutex and may come from any OS thread.
  */
 #ifndef GARECON_H
@@ -53,7 +53,7 @@ typedef uint64_t gar_str; /* bits 0..39 byte offset into the slab, bits 40..63 l
 typedef enum {
   GAR_OK = 0,
   GAR_E_INVALID = -1,  /* bad argument / malformed table (offset out of slab, non-monotone CSR ...) */
-  GAR_E_NO_DEVICE = -2,/* no CUDA device, or device is not sm_100 */
+  GAR_E_NO_DEVICE = -2,/* no CUDA device, or device is not sm_90 */
   GAR_E_CUDA = -3,     /* a CUDA call failed; text in gar_last_error */
   GAR_E_STATE = -4,    /* call order wrong (diff before load ...) */
   GAR_E_NOMEM = -5
@@ -336,7 +336,7 @@ typedef struct gar_engine gar_engine;
 
 /* ---------------------------------------------------------------- entry points */
 
-/* Create an engine bound to one CUDA device.  Fails with GAR_E_NO_DEVICE when there is no sm_100 GPU. */
+/* Create an engine bound to one CUDA device.  Fails with GAR_E_NO_DEVICE when there is no sm_90 GPU. */
 int gar_engine_create(const gar_config *cfg, gar_engine **out);
 void gar_engine_destroy(gar_engine *e);
 
@@ -474,7 +474,7 @@ uint64_t gar_shard_blob_bytes(const uint64_t *meta_row);
    RECEIVE arenas of the other GPUs through CUDA IPC; gar_shard_pack_peers packs the rank's own blob in place and the others into a
    local stage from which a copy kernel on a high-priority stream pushes them into the peers' arenas over NVLink (16-byte coalesced
    stores), level group by level group while the later levels are still being packed (transfer and partitioning overlap).
-   Alternatives kept behind environment switches because they were measured and lost on 8 B200s: GAR_PEER_CE=1 (copy engines
+   Alternatives kept behind environment switches for measurement: GAR_PEER_CE=1 (copy engines
    instead of the copy kernel), GAR_PEER_DIRECT=1 (the pack kernels store straight into the mapped arenas: 8-byte scattered
    stores over NVLink), GAR_PACK_TMA=1 (bulk stores from shared memory).  Per round:
 

@@ -1,5 +1,5 @@
-"""Why does gar_snapshot_load see 47 GB/s when one big pinned copy reaches 55 GB/s on this box?  Compares
-(A) generator buffers pinned in place with cudaHostRegister, (B) the same tables copied into cudaHostAlloc memory."""
+"""Host-to-device rate of gar_snapshot_load for the same tables in three placements: pageable, copied into cudaHostAlloc
+memory, and generator buffers pinned in place with cudaHostRegister (what bench.py's end-to-end arm does)."""
 import ctypes as C
 import importlib
 import sys

@@ -12,7 +12,7 @@ if str(REPO / "tests") not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (sm_90); select with -m gpu")
 
 
 @pytest.fixture(scope="session")

@@ -1,6 +1,6 @@
 // hostsim.cpp — TEST BUILD ONLY: the engine's row logic and pipeline (csrc/gar_rows.h, gar_pipeline.h) compiled
 // for the host, with loops / std::stable_sort standing in for kernels.  It exists because the build container has
-// no GPU: it lets `pytest -m "not gpu"` run the very functions the sm_100a kernels are made of against the oracle.
+// no GPU: it lets `pytest -m "not gpu"` run the very functions the sm_90a kernels are made of against the oracle.
 // It is never loaded by the package and is not a fallback: libgarecon.so has no CPU path.
 #include <algorithm>
 #include <cstdlib>

@@ -1,5 +1,5 @@
 """The bench contract's reference arm (`bench.py --impl reference`) runs on the host cores only: its JSON line can be checked on
-the CPU tier.  (The GPU arm of bench.py needs a B200 and is exercised by the driver / `gpurun`.)"""
+the CPU tier.  (The GPU arm of bench.py needs an H100.)"""
 import json
 import subprocess
 import sys

@@ -5,7 +5,7 @@ diff of every single-lbIngress object must be empty (statuses that are waiting s
 several lbIngress hostnames flip-flop in the reference too (each lbIngress rewrites the same accelerator,
 global_accelerator.go:150-156), so they are excluded from the fixed-point assertion, not from parity.
 
-The CPU tier runs it with the oracle and the warp-emulating hostsim build; the GPU tier with the sm_100a library."""
+The CPU tier runs it with the oracle and the warp-emulating hostsim build; the GPU tier with the sm_90a library."""
 import copy
 
 import numpy as np

@@ -1,4 +1,4 @@
-"""GPU tier: the sm_100a library, called through the C ABI (ctypes), must produce the oracle's change set
+"""GPU tier: the sm_90a library, called through the C ABI (ctypes), must produce the oracle's change set
 bit for bit (integer/index work: no tolerance)."""
 import numpy as np
 import pytest

@@ -1,6 +1,6 @@
 """CPU tier: the device row logic + pipeline (csrc/gar_rows.h, gar_pipeline.h) compiled for the host
 (tests/hostsim, a test build) must produce the oracle's change set bit for bit.  The same comparison runs
-against the real sm_100a library in test_gpu_parity.py."""
+against the real sm_90a library in test_gpu_parity.py."""
 import ctypes as C
 
 import pytest

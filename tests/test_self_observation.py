@@ -4,7 +4,7 @@ per-key loop re-lists AWS between iterations (global_accelerator.go:133-157, :98
 
 Pinned three ways: expectations derived by hand from the Go source; oracle/pyref.py, which SIMULATES the reference literally
 (an object-local overlay of everything its ops changed, every list call re-evaluated on it) against the closed-form rules of
-oracle/oracle.cpp; and the device code (hostsim here, the sm_100a library in the GPU tier) against the oracle."""
+oracle/oracle.cpp; and the device code (hostsim here, the sm_90a library in the GPU tier) against the oracle."""
 import importlib
 
 import numpy as np

@@ -357,7 +357,7 @@ def test_an_engine_error_on_one_rank_aborts_every_rank():
 
 @pytest.mark.gpu
 def test_nccl_ranks_equal_unsharded():
-    """One process per GPU, blobs over NCCL: needs >= 2 GPUs (the single-GPU test box skips it; run with gpurun --gpus N)."""
+    """One process per GPU, blobs over NCCL: needs >= 2 GPUs (skipped on a single-GPU machine)."""
     import torch
     n = torch.cuda.device_count()
     if n < 2:
@@ -369,7 +369,7 @@ def test_nccl_ranks_equal_unsharded():
     assert d["ok"] and d["n_ops"] > 100_000 and min(d["sent"]) > 0
 
 
-# ------------------------------------------------------------------ GPU tier: several engines on one B200, blobs in HBM
+# ------------------------------------------------------------------ GPU tier: several engines on one GPU, blobs in HBM
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("seed,n_ranks", [(0, 2), (1, 3), (2, 4), (3, 8), (4, 1)])
