@@ -107,6 +107,23 @@ class GarBindings(C.Structure):
     ]
 
 
+class GarObjectDelta(C.Structure):
+    _fields_ = [("upserts", C.POINTER(GarObjects)), ("n_deleted", C.c_uint32), ("deleted_kind", _u8p), ("deleted_key", C.POINTER(C.c_char_p))]
+
+
+class GarDeltaResult(C.Structure):
+    _fields_ = [("upsert_row", _u32p), ("deleted_row", _u32p), ("moved_from", _u32p), ("n_objects", C.c_uint32), ("slab_base", C.c_uint64),
+                ("slab_len", C.c_uint64)]
+
+
+class DeltaResult:
+    """Outcome of one object delta (include/garecon.h gar_delta_result), as numpy arrays."""
+
+    def __init__(self, upsert_row, deleted_row, moved_from, n_objects, slab_base, slab_len):
+        self.upsert_row, self.deleted_row, self.moved_from = upsert_row, deleted_row, moved_from
+        self.n_objects, self.slab_base, self.slab_len = int(n_objects), int(slab_base), int(slab_len)
+
+
 EGB_DELETING, EGB_HAS_FINALIZERS, EGB_OBSERVED = 1, 2, 4
 (OP_EGB_ADD_FINALIZER, OP_EGB_REMOVE_FINALIZER, OP_EGB_REMOVE_ENDPOINT, OP_EGB_ADD_ENDPOINT, OP_EGB_UPDATE_WEIGHT, OP_EGB_UPDATE_STATUS) = range(11, 17)
 ST_REQUEUE_1S = 8
@@ -255,6 +272,8 @@ def load_library(path: os.PathLike | None = None) -> C.CDLL:
     lib.gar_diff_keys.restype = C.c_int
     lib.gar_bindings_diff.argtypes = [C.c_void_p, C.POINTER(GarBindings), C.POINTER(GarChangeset)]
     lib.gar_bindings_diff.restype = C.c_int
+    lib.gar_snapshot_apply_objects.argtypes = [C.c_void_p, C.POINTER(GarObjectDelta), C.POINTER(GarDeltaResult)]
+    lib.gar_snapshot_apply_objects.restype = C.c_int
     lib.gar_shard_route.argtypes = [C.c_void_p, C.POINTER(GarShard), C.c_int, _u64p, _u64p]
     lib.gar_shard_route.restype = C.c_int
     lib.gar_shard_pack.argtypes = [C.c_void_p, C.c_void_p]
@@ -288,7 +307,7 @@ def load_library(path: os.PathLike | None = None) -> C.CDLL:
 
 EXPORTED_SYMBOLS = (
     "gar_engine_create", "gar_engine_destroy", "gar_snapshot_load", "gar_snapshot_attach_device", "gar_diff",
-    "gar_diff_device", "gar_diff_keys", "gar_bindings_diff", "gar_shard_route", "gar_shard_pack", "gar_shard_unpack", "gar_shard_blob_bytes",
+    "gar_diff_device", "gar_diff_keys", "gar_bindings_diff", "gar_snapshot_apply_objects", "gar_shard_route", "gar_shard_pack", "gar_shard_unpack", "gar_shard_blob_bytes",
     "gar_shard_arena", "gar_shard_open_peers", "gar_shard_pack_peers",
     "gar_changeset_free", "gar_last_error", "gar_version", "gar_algorithmic_bytes",
     "gar_last_stage_timings", "gar_last_counters",
@@ -349,6 +368,21 @@ class Engine:
         finally:
             self.lib.gar_changeset_free(self._h, C.byref(cs))
         return out
+
+    def apply_objects(self, upserts: GarObjects | None = None, deleted=()) -> DeltaResult:
+        """Object delta against the loaded snapshot (include/garecon.h gar_snapshot_apply_objects).  `upserts`: a GarObjects of
+        added / updated objects, e.g. tables.pack(objects, None).objects (its buffers must stay alive for the call);
+        `deleted`: [(kind, "ns/name"), ...].  Deletes run first, then upserts; each key at most once."""
+        nu = int(upserts.n_objects) if upserts is not None else 0
+        kinds = np.ascontiguousarray(np.asarray([k for k, _ in deleted] or [0], dtype=np.uint8))
+        keys = (C.c_char_p * max(1, len(deleted)))(*[s.encode() for _, s in deleted])
+        d = GarObjectDelta(C.pointer(upserts) if upserts is not None else None, len(deleted), kinds.ctypes.data_as(_u8p), C.cast(keys, C.POINTER(C.c_char_p)))
+        up_row = np.zeros(max(1, nu), dtype=np.uint32)
+        del_row = np.zeros(max(1, len(deleted)), dtype=np.uint32)
+        moved = np.zeros(max(1, len(deleted)), dtype=np.uint32)
+        res = GarDeltaResult(up_row.ctypes.data_as(_u32p), del_row.ctypes.data_as(_u32p), moved.ctypes.data_as(_u32p), 0, 0, 0)
+        self._check(self.lib.gar_snapshot_apply_objects(self._h, C.byref(d), C.byref(res)))
+        return DeltaResult(up_row[:nu].copy(), del_row[:len(deleted)].copy(), moved[:len(deleted)].copy(), res.n_objects, res.slab_base, res.slab_len)
 
     def bindings_diff(self, bindings) -> ChangeSet:
         """EndpointGroupBinding set-diff against the loaded snapshot; `bindings` has a .struct (GarBindings)."""

@@ -1,0 +1,415 @@
+// gar_delta.h — object deltas (gar_snapshot_apply_objects): informer events applied to the resident object table.
+//
+// Shared by the CUDA backend (gar_engine.cu) and the host simulation (tests/hostsim), like gar_shard.h: functors for the
+// data-parallel steps plus a driver template, Splicer<B>, that runs them over a Backend.  Data movement of one delta:
+//   1. the keys of the delta (deletes, then upserts) are resolved against the resident ix_obj index on the device, one
+//      thread per key with a full key compare after the tag (as object_in_cache does);
+//   2. the host turns the resolved rows into the delete / swap-move / replace / append sequence of include/garecon.h:
+//      O(batch) work that yields a short list of (new row <- source) overrides on top of the identity map;
+//   3. the upsert table is copied to the device; its slab is appended to the resident object slab (16-byte aligned);
+//   4. the object table is re-laid out dense into the standby column set: source map, per-row child counts + one scan per
+//      CSR, then a gather of the fixed-width columns and a warp-cooperative copy of the child rows (string references of
+//      rows that come from the upsert batch are rebased by the slab offset).  The standby set then becomes the resident one.
+// Re-laying instead of keeping (begin, end) pairs per row means every decision kernel keeps reading x_begin[i + 1] and
+// gar_rows.h does not change.  The pipeline's object side is marked stale and rebuilt by the next diff (gar_pipeline.h).
+//
+// Backend interface, on top of gar_pipeline.h's:
+//   void upload(void *dev_dst, const void *host_src, size_t bytes);
+//   void *delta_scratch(int k, size_t bytes);          // staging buffer k (DS_*)
+//   void *delta_col(int c, size_t bytes);              // column c (DC_*) of the STANDBY object column set
+//   void delta_swap();                                 // the standby set becomes the resident one
+//   u8 *delta_slab(u64 keep, u64 need);                // resident object slab with >= need bytes, the first `keep` preserved
+#pragma once
+
+#include <string.h>
+
+#include <algorithm>
+#include <string>
+#include <unordered_map>
+#include <unordered_set>
+#include <vector>
+
+#include "gar_pipeline.h"
+
+// object table columns, in gar_objects order (also the order in which gar_snapshot_load uploads them)
+enum DeltaCol {
+  DC_KIND, DC_SPEC, DC_FLAGS, DC_NS, DC_NAME, DC_ICLS, DC_ANN_B, DC_LBI_B, DC_PORT_B, DC_ANN_KEY, DC_ANN_VAL, DC_LBI_HOST, DC_PORT_NUM,
+  DC_PORT_PROTO, DC_N
+};
+// staging buffers: the upsert columns (DS_UP + DC_*), keys, source map
+enum DeltaScratch { DS_UP = 0, DS_KEY_KIND = DC_N, DS_KEY_REF, DS_KEY_SLAB, DS_COUNTS, DS_OFFS, DS_ROWS, DS_PAIRS, DS_SRC, DS_TOTALS, DS_N };
+
+constexpr u32 SRC_UPSERT = 0x80000000u;  // source map: row of the upsert batch (else a row of the resident table)
+
+// all rows of the resident table that carry key k (kind + "ns/name"); count pass (rows == nullptr), then write pass.
+// Entries of an ix_obj bucket are ordered by row, so the rows come out ascending.
+struct FDeltaResolve {
+  DevTables T;
+  HashIdx ix;
+  const u8 *kind;
+  const gar_str *key;
+  const u8 *slab;
+  u32 *counts;
+  const u32 *offs;
+  u32 *rows;
+  GAR_HD void operator()(u32 k) const {
+    const u32 kd = kind[k];
+    const Str ks = mkstr(slab, key[k]);
+    Cursor c = idx_open(ix, key_hash_kinded(kd, ks));
+    IdxEntry e;
+    u32 m = 0;
+    while (idx_next(ix, c, &e))
+      if (e.a0 == kd && streq(mkstr(T.o.slab, e.s0), ks)) {
+        if (rows) rows[offs[k] + m] = e.row;
+        m++;
+      }
+    if (!rows) counts[k] = m;
+  }
+};
+struct FDeltaIdentity {
+  u32 *src;
+  GAR_HD void operator()(u32 i) const { src[i] = i; }
+};
+struct FDeltaScatter {
+  const u32 *pairs;  // (new row, source) pairs
+  u32 *src;
+  GAR_HD void operator()(u32 k) const { src[pairs[2 * k]] = pairs[2 * k + 1]; }
+};
+// the output side of a splice: the standby columns
+struct DeltaOut {
+  u8 *kind, *spec, *flags;
+  gar_str *ns, *name, *icls;
+  u32 *ann_b, *lbi_b, *port_b;
+  gar_str *ann_key, *ann_val, *lbi_host, *port_proto;
+  i32 *port_num;
+};
+// new row i: fixed-width columns from its source row, and its child counts (row n: the 0 that becomes the scans' total)
+struct FDeltaRows {
+  gar_objects R, U;  // resident table, upsert batch (device copies)
+  const u32 *src;
+  u64 base;          // slab offset of the upsert batch's strings
+  u32 n;
+  DeltaOut D;
+  GAR_HD void operator()(u32 i) const {
+    if (i == n) {
+      D.ann_b[n] = D.lbi_b[n] = D.port_b[n] = 0;
+      return;
+    }
+    const u32 s = src[i], r = s & ~SRC_UPSERT;
+    const bool up = (s & SRC_UPSERT) != 0;
+    const gar_objects &S = up ? U : R;
+    const u64 rb = up ? base : 0;
+    const u8 fl = S.obj_flags[r];
+    D.kind[i] = S.obj_kind[r];
+    D.spec[i] = S.obj_spec_type[r];
+    D.flags[i] = fl;
+    D.ns[i] = S.obj_ns[r] + rb;  // the offset lives in the low bits of a gar_str
+    D.name[i] = S.obj_name[r] + rb;
+    D.icls[i] = (fl & GAR_OBJ_HAS_INGRESS_CLASS) ? S.obj_ingress_class[r] + rb : S.obj_ingress_class[r];
+    D.ann_b[i] = S.obj_ann_begin[r + 1] - S.obj_ann_begin[r];
+    D.lbi_b[i] = S.obj_lbi_begin[r + 1] - S.obj_lbi_begin[r];
+    D.port_b[i] = S.obj_port_begin[r + 1] - S.obj_port_begin[r];
+  }
+};
+struct FDeltaTotals {
+  const u32 *ann, *lbi, *port;  // the scanned begins' last entries
+  u32 *out;
+  GAR_HD void operator()(u32) const {
+    out[0] = *ann;
+    out[1] = *lbi;
+    out[2] = *port;
+  }
+};
+// child rows: 32 consecutive threads (one warp on the GPU) per new row, striding over its children — a row with many
+// annotations or hostnames is not walked by one thread (DESIGN.md §4 "Skew")
+struct FDeltaChildren {
+  gar_objects R, U;
+  const u32 *src;
+  u64 base;
+  DeltaOut D;
+  GAR_HD void operator()(u32 t) const {
+    const u32 i = t >> 5, lane = t & 31u;
+    const u32 s = src[i], r = s & ~SRC_UPSERT;
+    const bool up = (s & SRC_UPSERT) != 0;
+    const gar_objects &S = up ? U : R;
+    const u64 rb = up ? base : 0;
+    {
+      const u32 d0 = D.ann_b[i], c = D.ann_b[i + 1] - d0, s0 = S.obj_ann_begin[r];
+      for (u32 k = lane; k < c; k += 32) {
+        D.ann_key[d0 + k] = S.ann_key[s0 + k] + rb;
+        D.ann_val[d0 + k] = S.ann_val[s0 + k] + rb;
+      }
+    }
+    {
+      const u32 d0 = D.lbi_b[i], c = D.lbi_b[i + 1] - d0, s0 = S.obj_lbi_begin[r];
+      for (u32 k = lane; k < c; k += 32) D.lbi_host[d0 + k] = S.lbi_hostname[s0 + k] + rb;
+    }
+    {
+      const u32 d0 = D.port_b[i], c = D.port_b[i + 1] - d0, s0 = S.obj_port_begin[r];
+      for (u32 k = lane; k < c; k += 32) {
+        D.port_num[d0 + k] = S.port_number[s0 + k];
+        D.port_proto[d0 + k] = S.port_proto[s0 + k] + rb;
+      }
+    }
+  }
+};
+
+// ------------------------------------------------------------------ host-side checks of the (small) upsert batch
+
+// the checks gar_snapshot_load runs on the device, for a table the host holds; "" = valid
+inline std::string delta_check_upserts(const gar_objects &o) {
+  const u32 n = o.n_objects;
+  if (!n) return "";
+  if (!o.obj_kind || !o.obj_spec_type || !o.obj_flags || !o.obj_ns || !o.obj_name || !o.obj_ingress_class || !o.obj_ann_begin || !o.obj_lbi_begin ||
+      !o.obj_port_begin || (o.n_ann && (!o.ann_key || !o.ann_val)) || (o.n_lbi && !o.lbi_hostname) || (o.n_ports && (!o.port_number || !o.port_proto)) ||
+      (o.slab_len && !o.slab))
+    return "upserts: NULL column";
+  auto str_ok = [&](gar_str r) { return GAR_STR_OFF(r) + GAR_STR_LEN(r) <= o.slab_len; };
+  auto csr_ok = [&](const u32 *b, u32 nchildren) {
+    if (b[0] != 0 || b[n] != nchildren) return false;
+    for (u32 i = 0; i < n; i++)
+      if (b[i + 1] < b[i]) return false;
+    return true;
+  };
+  if (!csr_ok(o.obj_ann_begin, o.n_ann)) return "upserts: obj_ann_begin: CSR is not monotone, does not start at 0 or does not end at the child count";
+  if (!csr_ok(o.obj_lbi_begin, o.n_lbi)) return "upserts: obj_lbi_begin: CSR is not monotone, does not start at 0 or does not end at the child count";
+  if (!csr_ok(o.obj_port_begin, o.n_ports)) return "upserts: obj_port_begin: CSR is not monotone, does not start at 0 or does not end at the child count";
+  for (u32 i = 0; i < n; i++) {
+    if (o.obj_kind[i] > GAR_KIND_INGRESS || o.obj_spec_type[i] > GAR_SVC_EXTERNALNAME) return "upserts: obj_kind / obj_spec_type out of range";
+    if (!str_ok(o.obj_ns[i]) || !str_ok(o.obj_name[i])) return "upserts: obj_ns / obj_name: string reference outside the slab";
+    if ((o.obj_flags[i] & GAR_OBJ_HAS_INGRESS_CLASS) && !str_ok(o.obj_ingress_class[i])) return "upserts: obj_ingress_class: string reference outside the slab";
+    const u64 sep = GAR_STR_OFF(o.obj_ns[i]) + GAR_STR_LEN(o.obj_ns[i]);
+    if (GAR_STR_OFF(o.obj_name[i]) != sep + 1 || sep >= o.slab_len || o.slab[sep] != '/')
+      return "upserts: objects layout rule violated: obj_ns and obj_name must be slices of one \"ns/name\" key string";
+  }
+  for (u32 k = 0; k < o.n_ann; k++)
+    if (!str_ok(o.ann_key[k]) || !str_ok(o.ann_val[k])) return "upserts: ann_key / ann_val: string reference outside the slab";
+  for (u32 k = 0; k < o.n_lbi; k++)
+    if (!str_ok(o.lbi_hostname[k])) return "upserts: lbi_hostname: string reference outside the slab";
+  for (u32 k = 0; k < o.n_ports; k++)
+    if (!str_ok(o.port_proto[k])) return "upserts: port_proto: string reference outside the slab";
+  return "";
+}
+
+// ------------------------------------------------------------------ the driver
+
+// B: the backend the splice runs on; PB: the backend of the engine's Pipeline (the same one, unless B adds the delta buffers
+// to an existing backend, as the host simulation does)
+template <class B, class PB = B>
+struct Splicer {
+  B &be;
+  Pipeline<PB> &P;
+  DevTables &T;  // the resident tables: T.o is replaced by a splice
+  std::string error;
+
+  template <class Tp>
+  const Tp *up(int k, const Tp *host, size_t count) {
+    const size_t bytes = count * sizeof(Tp);
+    void *p = be.delta_scratch(k, bytes + GAR_SLAB_PAD + 16);
+    if (bytes) be.upload(p, host, bytes);
+    return (const Tp *)p;
+  }
+
+  // GAR_OK, GAR_E_INVALID (error says why; nothing changed) or another gar_rc
+  int apply(const gar_object_delta &d, gar_delta_result &out) {
+    static const gar_objects kNoUpserts{};
+    const gar_objects &U = (d.upserts && d.upserts->n_objects) ? *d.upserts : kNoUpserts;
+    const u32 nu = U.n_objects, nd = d.n_deleted, nk = nd + nu;
+    if ((nu && !out.upsert_row) || (nd && (!out.deleted_row || !out.moved_from))) return invalid("NULL result array");
+    if (nd && (!d.deleted_kind || !d.deleted_key)) return invalid("NULL deleted-key arrays");
+    error = delta_check_upserts(U);
+    if (!error.empty()) return GAR_E_INVALID;
+    // the keys, deletes first: kind + "ns/name" in one host slab; every key at most once
+    std::vector<u8> kind(nk + 1, 0), kslab;
+    std::vector<gar_str> kref(nk + 1, 0);
+    std::unordered_set<std::string> seen;
+    for (u32 k = 0; k < nk; k++) {
+      const char *p;
+      size_t len;
+      if (k < nd) {
+        if (!d.deleted_key[k] || d.deleted_kind[k] > GAR_KIND_INGRESS) return invalid("bad deleted key");
+        kind[k] = d.deleted_kind[k];
+        p = d.deleted_key[k];
+        len = strlen(p);
+      } else {
+        const u32 u = k - nd;
+        kind[k] = U.obj_kind[u];
+        p = (const char *)U.slab + GAR_STR_OFF(U.obj_ns[u]);
+        len = GAR_STR_LEN(U.obj_ns[u]) + 1 + GAR_STR_LEN(U.obj_name[u]);
+      }
+      std::string key(1, (char)('0' + kind[k]));
+      key.append(p, len);
+      if (!seen.insert(key).second) return invalid("a key appears twice in one delta (deletes and upserts together): coalesce the events first");
+      kref[k] = GAR_STR(kslab.size(), len);
+      kslab.insert(kslab.end(), p, p + len);
+    }
+    const u64 base = nu ? (T.o.slab_len + 15) & ~(u64)15 : 0;
+    if (nu && base + U.slab_len + GAR_SLAB_PAD >= (1ull << GAR_STR_OFF_BITS)) return invalid("the resident object slab would outgrow 2^40 bytes: reload");
+    if ((u64)T.o.n_objects + nu >= (1u << 27)) return invalid("too many objects for one snapshot");
+    out.n_objects = T.o.n_objects;
+    out.slab_base = base;
+    out.slab_len = T.o.slab_len;
+    if (!nk) return GAR_OK;
+
+    // 1. resolve every key against ix_obj: all rows that carry it, ascending
+    int rc = P.index_objects();
+    if (rc != GAR_OK) return invalid("the resident object table could not be indexed");
+    kslab.resize(kslab.size() + GAR_SLAB_PAD, 0);
+    const u8 *dkind = up(DS_KEY_KIND, kind.data(), nk);
+    const gar_str *dref = up(DS_KEY_REF, kref.data(), nk);
+    const u8 *dkslab = up(DS_KEY_SLAB, kslab.data(), kslab.size());
+    u32 *dcounts = (u32 *)be.delta_scratch(DS_COUNTS, 4 * (size_t)(nk + 1));
+    be.for_each("delta_resolve", nk, FDeltaResolve{T, P.W.ix_obj, dkind, dref, dkslab, dcounts, nullptr, nullptr});
+    std::vector<u32> counts(nk), offs(nk + 1, 0);
+    be.download(counts.data(), dcounts, 4 * (size_t)nk);
+    for (u32 k = 0; k < nk; k++) offs[k + 1] = offs[k] + counts[k];
+    std::vector<u32> match(offs[nk] + 1);
+    if (offs[nk]) {
+      const u32 *doffs = up(DS_OFFS, offs.data(), nk + 1);
+      u32 *drows = (u32 *)be.delta_scratch(DS_ROWS, 4 * (size_t)(offs[nk] + 1));
+      be.for_each("delta_resolve", nk, FDeltaResolve{T, P.W.ix_obj, dkind, dref, dkslab, dcounts, doffs, drows});
+      be.download(match.data(), drows, 4 * (size_t)offs[nk]);
+    }
+
+    // 2. the delete / move / replace / append sequence (include/garecon.h), on rows of the resident table ("orig" rows)
+    u32 n = T.o.n_objects;
+    std::unordered_map<u32, u32> orig_at, cur_of;  // moved rows only: current row -> orig row, orig row -> current row
+    std::unordered_set<u32> gone;                  // orig rows deleted
+    auto lowest = [&](u32 k) {
+      u32 best = GAR_NONE;
+      for (u32 m = offs[k]; m < offs[k + 1]; m++) {
+        const u32 o = match[m];
+        if (gone.count(o)) continue;
+        auto it = cur_of.find(o);
+        best = std::min(best, it == cur_of.end() ? o : it->second);
+      }
+      return best;
+    };
+    auto orig = [&](u32 row) {
+      auto it = orig_at.find(row);
+      return it == orig_at.end() ? row : it->second;
+    };
+    for (u32 k = 0; k < nd; k++) {
+      const u32 r = lowest(k);
+      out.deleted_row[k] = r;
+      out.moved_from[k] = GAR_NONE;
+      if (r == GAR_NONE) continue;
+      const u32 last = n - 1, o_r = orig(r);
+      gone.insert(o_r);
+      cur_of.erase(o_r);
+      if (r != last) {
+        const u32 o_last = orig(last);
+        orig_at[r] = o_last;
+        cur_of[o_last] = r;
+        out.moved_from[k] = last;
+      }
+      orig_at.erase(last);
+      n--;
+    }
+    std::unordered_map<u32, u32> src_at(orig_at.begin(), orig_at.end());  // new row -> source, where not the identity
+    for (u32 u = 0; u < nu; u++) {
+      u32 r = lowest(nd + u);
+      if (r == GAR_NONE) r = n++;
+      src_at[r] = SRC_UPSERT | u;
+      out.upsert_row[u] = r;
+    }
+    out.n_objects = n;
+    if (src_at.empty() && n == T.o.n_objects) return GAR_OK;  // only absent keys: nothing moves
+
+    // 3. the upsert batch on the device; its strings behind the resident ones
+    gar_objects DU{};
+    u8 *slab = (u8 *)T.o.slab;
+    u64 slab_len = T.o.slab_len;
+    if (nu) {
+      DU = U;
+      DU.obj_kind = up(DS_UP + DC_KIND, U.obj_kind, nu);
+      DU.obj_spec_type = up(DS_UP + DC_SPEC, U.obj_spec_type, nu);
+      DU.obj_flags = up(DS_UP + DC_FLAGS, U.obj_flags, nu);
+      DU.obj_ns = up(DS_UP + DC_NS, U.obj_ns, nu);
+      DU.obj_name = up(DS_UP + DC_NAME, U.obj_name, nu);
+      DU.obj_ingress_class = up(DS_UP + DC_ICLS, U.obj_ingress_class, nu);
+      DU.obj_ann_begin = up(DS_UP + DC_ANN_B, U.obj_ann_begin, nu + 1);
+      DU.obj_lbi_begin = up(DS_UP + DC_LBI_B, U.obj_lbi_begin, nu + 1);
+      DU.obj_port_begin = up(DS_UP + DC_PORT_B, U.obj_port_begin, nu + 1);
+      DU.ann_key = up(DS_UP + DC_ANN_KEY, U.ann_key, U.n_ann);
+      DU.ann_val = up(DS_UP + DC_ANN_VAL, U.ann_val, U.n_ann);
+      DU.lbi_hostname = up(DS_UP + DC_LBI_HOST, U.lbi_hostname, U.n_lbi);
+      DU.port_number = up(DS_UP + DC_PORT_NUM, U.port_number, U.n_ports);
+      DU.port_proto = up(DS_UP + DC_PORT_PROTO, U.port_proto, U.n_ports);
+      slab_len = base + U.slab_len;
+      slab = be.delta_slab(T.o.slab_len, slab_len + GAR_SLAB_PAD);
+      static const u8 kZeros[GAR_SLAB_PAD] = {};
+      if (U.slab_len) be.upload(slab + base, U.slab, U.slab_len);
+      be.upload(slab + slab_len, kZeros, GAR_SLAB_PAD);
+    }
+    gar_objects R = T.o;
+    R.slab = slab;
+
+    // 4. the dense re-layout into the standby set
+    std::vector<u32> pairs;
+    pairs.reserve(2 * src_at.size());
+    for (auto &kv : src_at) {
+      pairs.push_back(kv.first);
+      pairs.push_back(kv.second);
+    }
+    u32 *dsrc = (u32 *)be.delta_scratch(DS_SRC, 4 * (size_t)(n + 1));
+    if (n) be.for_each("delta_source_map", n, FDeltaIdentity{dsrc});
+    if (!pairs.empty()) be.for_each("delta_source_map", (u32)src_at.size(), FDeltaScatter{up(DS_PAIRS, pairs.data(), pairs.size()), dsrc});
+    DeltaOut D{};
+    D.kind = (u8 *)be.delta_col(DC_KIND, (size_t)n + 16);
+    D.spec = (u8 *)be.delta_col(DC_SPEC, (size_t)n + 16);
+    D.flags = (u8 *)be.delta_col(DC_FLAGS, (size_t)n + 16);
+    D.ns = (gar_str *)be.delta_col(DC_NS, 8 * (size_t)n + 16);
+    D.name = (gar_str *)be.delta_col(DC_NAME, 8 * (size_t)n + 16);
+    D.icls = (gar_str *)be.delta_col(DC_ICLS, 8 * (size_t)n + 16);
+    D.ann_b = (u32 *)be.delta_col(DC_ANN_B, 4 * (size_t)(n + 1) + 16);
+    D.lbi_b = (u32 *)be.delta_col(DC_LBI_B, 4 * (size_t)(n + 1) + 16);
+    D.port_b = (u32 *)be.delta_col(DC_PORT_B, 4 * (size_t)(n + 1) + 16);
+    be.for_each("delta_rows", n + 1, FDeltaRows{R, DU, dsrc, base, n, D});
+    be.exclusive_scan(D.ann_b, n + 1);
+    be.exclusive_scan(D.lbi_b, n + 1);
+    be.exclusive_scan(D.port_b, n + 1);
+    u32 *dtot = (u32 *)be.delta_scratch(DS_TOTALS, 64);
+    be.for_each("delta_totals", 1, FDeltaTotals{D.ann_b + n, D.lbi_b + n, D.port_b + n, dtot});
+    u32 tot[3];
+    be.download(tot, dtot, sizeof(tot));
+    D.ann_key = (gar_str *)be.delta_col(DC_ANN_KEY, 8 * (size_t)tot[0] + 16);
+    D.ann_val = (gar_str *)be.delta_col(DC_ANN_VAL, 8 * (size_t)tot[0] + 16);
+    D.lbi_host = (gar_str *)be.delta_col(DC_LBI_HOST, 8 * (size_t)tot[1] + 16);
+    D.port_num = (i32 *)be.delta_col(DC_PORT_NUM, 4 * (size_t)tot[2] + 16);
+    D.port_proto = (gar_str *)be.delta_col(DC_PORT_PROTO, 8 * (size_t)tot[2] + 16);
+    if (n) be.for_each("delta_children", n * 32, FDeltaChildren{R, DU, dsrc, base, D});
+    be.delta_swap();
+    gar_objects &O = T.o;
+    O.n_objects = n;
+    O.obj_kind = D.kind;
+    O.obj_spec_type = D.spec;
+    O.obj_flags = D.flags;
+    O.obj_ns = D.ns;
+    O.obj_name = D.name;
+    O.obj_ingress_class = D.icls;
+    O.obj_ann_begin = D.ann_b;
+    O.obj_lbi_begin = D.lbi_b;
+    O.obj_port_begin = D.port_b;
+    O.n_ann = tot[0];
+    O.ann_key = D.ann_key;
+    O.ann_val = D.ann_val;
+    O.n_lbi = tot[1];
+    O.lbi_hostname = D.lbi_host;
+    O.n_ports = tot[2];
+    O.port_number = D.port_num;
+    O.port_proto = D.port_proto;
+    O.slab = slab;
+    O.slab_len = slab_len;
+    P.T = T;
+    P.obj_stale = true;
+    out.slab_len = slab_len;
+    return GAR_OK;
+  }
+
+ private:
+  int invalid(const char *msg) {
+    error = msg;
+    return GAR_E_INVALID;
+  }
+};

@@ -24,6 +24,7 @@
 
 #include "gar_pipeline.h"
 #include "gar_shard.h"
+#include "gar_delta.h"
 
 #define GAR_VERSION_STRING "garecon 0.1.0 (sm_90a)"
 
@@ -853,6 +854,32 @@ struct gar_engine {
   void *out_dports(u64 n) { return dev_ensure(d_dports, 4 * (size_t)(n + 1)); }
   void *out_status_ga(u32 n) { return dev_ensure(d_status_ga, 4 * (size_t)(n + 1)); }
   void *out_status_r53(u32 n) { return dev_ensure(d_status_r53, 4 * (size_t)(n + 1)); }
+
+  // ---- object deltas (gar_delta.h).  The resident object columns live either in in[DC_*] (as gar_snapshot_load left them,
+  // o_set 0) or in dset[DC_*] (o_set 1); a splice writes the other set and then swaps.  The object slab stays in in[DC_N].
+  DBuf dset[DC_N], dscratch[DS_N];
+  int o_set = 0;
+  void upload(void *dst, const void *src, size_t bytes) {
+    if (bytes) CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, stream));
+  }
+  void *delta_scratch(int k, size_t bytes) { return dev_ensure(dscratch[k], bytes); }
+  void *delta_col(int c, size_t bytes) { return dev_ensure(o_set == 0 ? dset[c] : in[c], bytes); }
+  void delta_swap() { o_set ^= 1; }
+  u8 *delta_slab(u64 keep, u64 need) {
+    DBuf &b = in[DC_N];
+    if (b.cap < need + 16) {
+      graph_drop();
+      size_t want = (size_t)(need + need / 2 + 256) & ~(size_t)255;
+      void *p = nullptr;
+      CK(cudaMalloc(&p, want));
+      if (keep) CK(cudaMemcpyAsync(p, b.p, keep, cudaMemcpyDeviceToDevice, stream));
+      CK(cudaStreamSynchronize(stream));
+      CK(cudaFree(b.p));
+      b.p = p;
+      b.cap = want;
+    }
+    return (u8 *)b.p;
+  }
 };
 
 // ------------------------------------------------------------------ host-side checks of small tables (bindings) and of pointers
@@ -985,6 +1012,7 @@ static void do_load(gar_engine *e, const gar_objects *o, const gar_actual *a) {
   validate_pointers(o, a);  // NULL checks before anything is copied; the contents are checked on the device, below
   CK(cudaSetDevice(e->device));
   e->in_used = 0;
+  e->o_set = 0;  // the object columns go to in[DC_*] again
   DevTables &T = e->T;
   CK(cudaEventRecord(e->ev[0], e->stream));
   T.o = *o;
@@ -1045,6 +1073,54 @@ static void do_load(gar_engine *e, const gar_objects *o, const gar_actual *a) {
 
 // ------------------------------------------------------------------ diff
 
+// the prepared state of the loaded snapshot (digests, indexes) lives as long as the snapshot
+static Pipeline<gar_engine> &ensure_pipe(gar_engine *e) {
+  if (!e->pipe) {
+    e->graph_drop();  // recorded launches belong to the previous pipeline's buffers and tables
+    e->pipe = new Pipeline<gar_engine>(*e, e->T);
+    if (const char *tc = getenv("GAR_TINY_CAPS")) e->pipe->tiny_caps = tc[0] == '1';
+    if (!e->pipe->tiny_caps) {
+      e->pipe->dport_cap = e->hint_dport_cap;
+      e->pipe->pair_cap = e->hint_pair_cap;
+      e->pipe->ops_cap = e->hint_ops_cap;
+    }
+    if (e->shard_home) {
+      e->pipe->acc_guest_from = e->sharder->guest_from;
+      e->pipe->sharded = 1;
+    }
+  }
+  return *e->pipe;
+}
+
+// ------------------------------------------------------------------ object deltas
+
+static void do_apply(gar_engine *e, const gar_object_delta *d, gar_delta_result *out) {
+  if (!e->loaded) throw StateError{"no snapshot loaded"};
+  if (e->attached) throw StateError{"object deltas need a snapshot the engine owns: an attached (device) snapshot cannot be changed"};
+  if (e->shard_home || e->shard_round != 0) throw StateError{"object deltas are not available in sharded mode"};
+  CK(cudaSetDevice(e->device));
+  e->graph_drop();
+  e->marks.clear();
+  e->events_used = 0;
+  e->stage_depth = 0;
+  try {
+    Pipeline<gar_engine> &P = ensure_pipe(e);
+    Splicer<gar_engine> S{*e, P, e->T};
+    const int rc = S.apply(*d, *out);
+    CK(cudaStreamSynchronize(e->stream));
+    CK(cudaGetLastError());
+    if (rc == GAR_E_INVALID) throw InvalidError{S.error};
+    if (rc != GAR_OK) throw StateError{"the object delta could not be applied"};
+    e->slice = e->T;
+    e->input_bytes = table_bytes(&e->T.o, &e->T.a);  // counts and slab lengths only
+  } catch (const CudaError &) {
+    e->loaded = false;  // the splice may have stopped half-way: no snapshot until the next load
+    delete e->pipe;
+    e->pipe = nullptr;
+    throw;
+  }
+}
+
 static void do_diff(gar_engine *e, gar_changeset *out, bool to_host, const gar_keyset *ks = nullptr, const gar_bindings *bd = nullptr) {
   if (!e->loaded) throw InvalidError{"no snapshot loaded"};
   CK(cudaSetDevice(e->device));
@@ -1061,21 +1137,7 @@ static void do_diff(gar_engine *e, gar_changeset *out, bool to_host, const gar_k
   if (e->shard_home && e->shard_round != 4)
     throw StateError{"a new exchange has started: the previous sub-snapshot's strings live in receive buffers that are being refilled; "
                      "finish both rounds (gar_shard_unpack(.., 2, ..)) before the next diff"};
-  if (!e->pipe) {
-    e->graph_drop();  // recorded launches belong to the previous pipeline's buffers and tables
-    e->pipe = new Pipeline<gar_engine>(*e, e->T);
-    if (const char *tc = getenv("GAR_TINY_CAPS")) e->pipe->tiny_caps = tc[0] == '1';
-    if (!e->pipe->tiny_caps) {
-      e->pipe->dport_cap = e->hint_dport_cap;
-      e->pipe->pair_cap = e->hint_pair_cap;
-      e->pipe->ops_cap = e->hint_ops_cap;
-    }
-    if (e->shard_home) {
-      e->pipe->acc_guest_from = e->sharder->guest_from;
-      e->pipe->sharded = 1;
-    }
-  }
-  Pipeline<gar_engine> &P = *e->pipe;
+  Pipeline<gar_engine> &P = ensure_pipe(e);
   P.orphan_sweep = !e->no_orphans;
   P.allow_empty_cache = e->allow_empty_cache;
   if (e->reprepare) P.prepared = false;
@@ -1337,6 +1399,8 @@ void gar_engine_destroy(gar_engine *e) {
     for (auto &b : ar) cudaFree(b.p);
   for (DBuf *b : {&e->d_derived_keys, &e->d_key_rows, &e->d_del_kind, &e->d_del_key, &e->d_del_slab}) cudaFree(b->p);
   for (auto &b : e->d_egb) cudaFree(b.p);
+  for (auto &b : e->dset) cudaFree(b.p);
+  for (auto &b : e->dscratch) cudaFree(b.p);
   cudaFree(e->d_valid.p);
   for (int k = 0; k < 2; k++) {
     if (e->dl_pin[k].p) cudaFreeHost(e->dl_pin[k].p);
@@ -1402,6 +1466,11 @@ int gar_diff_keys(gar_engine *e, const gar_keyset *keys, gar_changeset *out) {
 int gar_bindings_diff(gar_engine *e, const gar_bindings *bindings, gar_changeset *out) {
   if (!out || !bindings) return GAR_E_INVALID;
   return guarded(e, [&] { do_diff(e, out, true, nullptr, bindings); });
+}
+
+int gar_snapshot_apply_objects(gar_engine *e, const gar_object_delta *d, gar_delta_result *out) {
+  if (!d || !out) return GAR_E_INVALID;
+  return guarded(e, [&] { do_apply(e, d, out); });
 }
 
 int gar_shard_route(gar_engine *e, const gar_shard *shard, int round, uint64_t *meta, uint64_t *send_bytes) {

@@ -538,6 +538,12 @@ struct FValueJoins {
     mark_orphan_value(T, W, v);
   }
 };
+// the object half of FValueJoins, alone: re-run after an object delta (the alias links read the actual side only)
+struct FMarkOrphanValue {
+  DevTables T;
+  Work W;
+  GAR_HD void operator()(u32 v) const { mark_orphan_value(T, W, v); }
+};
 
 // --- count / emit.  counts layout: [GA obj: n][GA orphan: nacc][R53 obj: n][orphan alias: nrec][orphan value: nval][total]
 struct CountLayout {
@@ -843,8 +849,9 @@ struct Pipeline {
   bool orphan_sweep = true;        // GAR_FLAG_NO_ORPHANS clears it
   bool allow_empty_cache = false;  // GAR_FLAG_ALLOW_EMPTY_CACHE
 
-  void alloc_work() {
-    const u32 n = T.o.n_objects, nlbi = T.o.n_lbi, nacc = T.a.n_accels, nrec = T.a.n_records, nval = T.a.n_values;
+  // per-object work arrays (the object side: sized by the object table, rebuilt after an object delta)
+  void alloc_obj_work() {
+    const u32 n = T.o.n_objects, nlbi = T.o.n_lbi;
     W.derived = (u32 *)be.ensure(S_DERIVED, 4 * (size_t)(n + 1));
     W.okey_hash = (u64 *)be.ensure(S_OKEY_HASH, 8 * (size_t)(n + 1));
     W.ann_r53 = (gar_str *)be.ensure(S_ANN_R53, 8 * (size_t)(n + 1));
@@ -855,6 +862,13 @@ struct Pipeline {
     W.tok_code = (u8 *)be.out_tok_code(nlbi);
     W.tok_name = (gar_str *)be.out_tok_name(nlbi);
     W.tok_region = (gar_str *)be.out_tok_region(nlbi);
+    W.r53_mode = (u8 *)be.ensure(S_R53_MODE, (size_t)n + 1);
+    W.r53_acc = (u32 *)be.ensure(S_R53_ACC, 4 * (size_t)(n + 1));
+    W.r53_acc_dns = (gar_str *)be.ensure(S_R53_ACC_DNS, 8 * (size_t)(n + 1));
+  }
+  void alloc_work() {
+    const u32 nacc = T.a.n_accels, nrec = T.a.n_records, nval = T.a.n_values;
+    alloc_obj_work();
     W.acc_flags = (u32 *)be.ensure(S_ACC_FLAGS, 4 * (size_t)(nacc + 1));
     W.acc_owner_key = (gar_str *)be.ensure(S_ACC_OWNER_KEY, 8 * (size_t)(nacc + 1));
     W.acc_owner = (gar_str *)be.ensure(S_ACC_OWNER, 8 * (size_t)(nacc + 1));
@@ -871,9 +885,6 @@ struct Pipeline {
     W.val_orphan = (u8 *)be.ensure(S_VAL_ORPHAN, nval + 1);
     W.val_link = (ValLink *)be.ensure(S_VAL_LINK, sizeof(ValLink) * (size_t)(nval + 1));
     W.acc_digest = (AccDigest *)be.ensure(S_ACC_DIGEST, sizeof(AccDigest) * (size_t)(nacc + 1));
-    W.r53_mode = (u8 *)be.ensure(S_R53_MODE, (size_t)n + 1);
-    W.r53_acc = (u32 *)be.ensure(S_R53_ACC, 4 * (size_t)(n + 1));
-    W.r53_acc_dns = (gar_str *)be.ensure(S_R53_ACC_DNS, 8 * (size_t)(n + 1));
     W.lb_hash = (u64 *)be.ensure(S_LB_HASH, 8 * (size_t)(T.a.n_lbs + 1));
     W.rec_flags = (u8 *)be.ensure(S_REC_FLAGS, (size_t)nrec + 1);
     for (int k = 0; k < IX_N; k++) W.hist[k] = IxHist{nullptr, 0};
@@ -1016,16 +1027,7 @@ struct Pipeline {
       arm_ovn();
     }
     stage1();
-    // stage 2: listen-ports annotation -> desired port lists (count, scan, write).  The total stays on the device: the list
-    // buffer has a capacity, a diff that needs more is re-run (run_with)
-    be.fill32(W.dport_begin, 0, (size_t)n + 1);
-    if (n) be.for_each("listen_ports_count", n, FJsonCount{T, W});
-    be.exclusive_scan(W.dport_begin, n + 1);
-    be.for_each("gather_header", 1, FGatherHeader{W.dport_begin + n, errflag});
-    if (dport_cap < n / 2 + 1024 && !(tiny_caps && dport_cap)) dport_cap = tiny_caps ? 1 : n / 2 + 1024;
-    W.dport_cap = dport_cap;
-    W.dports = (i32 *)be.out_dports(dport_cap);
-    if (n) be.for_each("listen_ports_write", n, FJsonWrite{T, W});
+    listen_ports();
 
     // stage 3: hash indexes
     u32 *overflow = errflag + FW_IDX_OVERFLOW;
@@ -1044,7 +1046,73 @@ struct Pipeline {
       if (nval) be.for_each("value_joins", nval, FValueJoins{T, W});
       W.ix_ovn = build_index(S_IX_OVN, nval, 8, FRowOvn{T, W}, overflow, true);
     }
+    obj_stale = ovn_stale = false;
     return GAR_OK;
+  }
+  // stage 2: listen-ports annotation -> desired port lists (count, scan, write).  The total stays on the device: the list
+  // buffer has a capacity, a diff that needs more is re-run (run_with)
+  void listen_ports() {
+    const u32 n = T.o.n_objects;
+    be.fill32(W.dport_begin, 0, (size_t)n + 1);
+    if (n) be.for_each("listen_ports_count", n, FJsonCount{T, W});
+    be.exclusive_scan(W.dport_begin, n + 1);
+    be.for_each("gather_header", 1, FGatherHeader{W.dport_begin + n, errflag});
+    if (dport_cap < n / 2 + 1024 && !(tiny_caps && dport_cap)) dport_cap = tiny_caps ? 1 : n / 2 + 1024;
+    W.dport_cap = dport_cap;
+    W.dports = (i32 *)be.out_dports(dport_cap);
+    if (n) be.for_each("listen_ports_write", n, FJsonWrite{T, W});
+  }
+
+  // ---- object deltas (gar_delta.h).  The prepared state splits in two halves:
+  //   actual side  digests, LB hashes, zone mask, records / values, the LB / owner / target-hostname / zone / value / alias
+  //                indexes and the value -> alias links: depend on the AWS tables only and stay resident across deltas;
+  //   object side  classify, tokenise, listen ports, ix_obj, and (for the full diff's orphan sweep only) the orphan value
+  //                marks + ix_ovn: rebuilt over the whole resident table after a delta.
+  // obj_stale: the object table changed since the object side was built.  ovn_stale: the orphan values lag behind ix_obj.
+  bool obj_stale = false, ovn_stale = false;
+  void prepare_objects() {
+    const u32 n = T.o.n_objects, nlbi = T.o.n_lbi;
+    alloc_obj_work();
+    be.fill32(errflag, 0, FW_WORDS);
+    W.hist[IX_OBJ] = IxHist{nullptr, 0};  // ix_obj is built on its own below: its size no longer fits the fused group-A arrays
+    u32 *derived_public = (u32 *)be.out_derived(n);
+    if (n) be.for_each("classify_objects", n, FClassify{T, W, derived_public, nullptr, errflag});
+    if (nlbi) be.for_each_staged("tokenise_hostnames", nlbi, FTokenise{T, W});
+    listen_ports();
+    W.ix_obj = build_index(S_IX_OBJ, n, 1, FRowObj{T, W}, errflag + FW_IDX_OVERFLOW, force_radix);
+    obj_stale = false;
+    ovn_stale = true;
+  }
+  void prepare_orphan_values() {
+    const u32 nval = T.a.n_values;
+    if (!force_radix) {
+      arm_ovn();
+      if (nval) be.for_each("orphan_values", nval, FMarkOrphanValue{T, W});
+      finish_ovn();
+    } else {
+      W.hist[IX_OVN] = IxHist{nullptr, 0};
+      if (nval) be.for_each("orphan_values", nval, FMarkOrphanValue{T, W});
+      W.ix_ovn = build_index(S_IX_OVN, nval, 8, FRowOvn{T, W}, errflag + FW_IDX_OVERFLOW, true);
+    }
+    ovn_stale = false;
+  }
+  // a complete ix_obj of the current object table (key resolution of a delta), with the same index-overflow fallback as run_with
+  int index_objects() {
+    for (int attempt = 0; attempt < 2; attempt++) {
+      if (!prepared) prepare();
+      else if (obj_stale) prepare_objects();
+      prepared = true;
+      u32 fl[FW_WORDS];
+      be.download(fl, errflag, sizeof(fl));
+      if (fl[FW_BAD_KEYS]) return GAR_E_INVALID;
+      if (fl[FW_IDX_OVERFLOW] && !force_radix) {
+        force_radix = true;
+        prepared = false;
+        continue;
+      }
+      return GAR_OK;
+    }
+    return GAR_E_STATE;
   }
 
   // route53 ensure in relational form over `slots` object slots (rows == nullptr: slot = object row).  The number of
@@ -1172,13 +1240,15 @@ struct Pipeline {
     for (int attempt = 0; attempt < 8; attempt++) {
       u64 sig = 0;
       if (full) {
-        sig = hmix(hmix(prepared ? 1 : 2, force_radix ? 3 : 4), hmix(hmix(dport_cap, pair_cap), ops_cap));
+        sig = hmix(hmix(prepared ? (obj_stale || ovn_stale ? 9 : 1) : 2, force_radix ? 3 : 4), hmix(hmix(dport_cap, pair_cap), ops_cap));
         sig = hmix(sig, hmix(orphan_sweep ? 5 : 6, tiny_caps ? 7 : 8)) | 1;
       }
       const int g = full ? be.graph_begin(sig) : 0;
       int rc = GAR_OK;
       if (g != 2) {
         if (!prepared) rc = prepare();
+        else if (obj_stale) prepare_objects();
+        if (rc == GAR_OK && full && ovn_stale) prepare_orphan_values();  // only the full diff's orphan sweep reads them
         if (rc == GAR_OK) rc = decide();
       }
       prepared = true;

@@ -1,0 +1,218 @@
+"""Object deltas at table level: the rules of gar_snapshot_apply_objects (include/garecon.h) on numpy column dicts, and a
+seeded churn generator of informer-like batches.
+
+ColumnMirror holds the object table a full gar_snapshot_load would need after a sequence of deltas, laid out like the
+engine's resident table: its slab is the loaded slab followed by every delta's upsert slab at a 16-byte aligned offset,
+so the mirror's string references (and therefore tok_name / tok_region of a diff) are bit-identical to the engine's.
+profiles/delta_bench.py and the GPU tests use both; the CPU tests use a dict-level mirror (tests/test_object_deltas.py).
+"""
+from __future__ import annotations
+
+import numpy as np
+
+from . import tables
+
+GAR_NONE = 0xFFFFFFFF
+_MASK = np.uint64((1 << 40) - 1)
+ANN_R53 = b"aws-global-accelerator-controller.h3poteto.dev/route53-hostname"
+ANN_LISTEN = b"alb.ingress.kubernetes.io/listen-ports"
+_CSRS = (("obj_ann_begin", ("ann_key", "ann_val")), ("obj_lbi_begin", ("lbi_hostname",)), ("obj_port_begin", ("port_number", "port_proto")))
+_FIXED = ("obj_kind", "obj_spec_type", "obj_flags", "obj_ns", "obj_name", "obj_ingress_class")
+
+
+def _off(refs):
+    return (refs & _MASK).astype(np.int64)
+
+
+def _len(refs):
+    return (refs >> np.uint64(40)).astype(np.int64)
+
+
+def take_rows(cols: dict, rows) -> dict:
+    """Object rows `rows` (in that order) of an object column dict; child rows follow their parents, the slab is shared."""
+    rows = np.asarray(rows, dtype=np.int64)
+    out = {c: np.asarray(cols[c])[rows] for c in _FIXED}
+    for bcol, children in _CSRS:
+        b = np.asarray(cols[bcol]).astype(np.int64)
+        cnt = b[rows + 1] - b[rows]
+        nb = np.concatenate([[0], np.cumsum(cnt)]).astype(np.int64)
+        idx = np.repeat(b[rows] - nb[:-1], cnt) + np.arange(nb[-1], dtype=np.int64)
+        out[bcol] = nb.astype(np.uint32)
+        for c in children:
+            out[c] = np.asarray(cols[c])[idx]
+    out["slab"] = cols["slab"]
+    return out
+
+
+def key_is(refs: np.ndarray, slab: np.ndarray, literal: bytes) -> np.ndarray:
+    """Mask of the gar_str references whose string equals `literal`."""
+    mask = _len(refs) == len(literal)
+    cand = np.flatnonzero(mask)
+    if len(cand) and literal:
+        o = _off(refs[cand])
+        same = (slab[o[:, None] + np.arange(len(literal))[None, :]] == np.frombuffer(literal, dtype=np.uint8)[None, :]).all(axis=1)
+        mask[cand[~same]] = False
+    return mask
+
+
+def row_keys(cols: dict) -> list:
+    """(kind, b"ns/name") of every object row."""
+    slab = np.asarray(cols["slab"])
+    off, ln = _off(cols["obj_ns"]), _len(cols["obj_ns"]) + 1 + _len(cols["obj_name"])
+    raw = slab.tobytes()
+    return [(int(k), raw[o:o + n]) for k, o, n in zip(cols["obj_kind"].tolist(), off.tolist(), ln.tolist())]
+
+
+def compact(cols: dict, new_keys=None) -> dict:
+    """A (small) object table with a slab of its own that holds exactly the strings it references.  new_keys[i] (optional,
+    bytes "ns/name" or None) renames row i."""
+    slab = np.asarray(cols["slab"])
+    out = {k: np.array(v, copy=True) for k, v in cols.items() if k != "slab"}
+    pieces = []
+    renamed = list(new_keys) if new_keys is not None else [None] * len(cols["obj_kind"])
+    kb = [nk if nk is not None else k for (_, k), nk in zip(row_keys(cols), renamed)]
+    ns_len = [k.index(b"/") if nk is not None else n for k, nk, n in zip(kb, renamed, _len(cols["obj_ns"]).tolist())]
+    blob = b"".join(kb)
+    koff = np.concatenate([[0], np.cumsum([len(k) for k in kb])]).astype(np.int64)
+    nsl = np.asarray(ns_len, dtype=np.int64)
+    out["obj_ns"] = (koff[:-1].astype(np.uint64)) | (nsl.astype(np.uint64) << np.uint64(40))
+    out["obj_name"] = ((koff[:-1] + nsl + 1).astype(np.uint64)) | ((koff[1:] - koff[:-1] - nsl - 1).astype(np.uint64) << np.uint64(40))
+    pieces.append(np.frombuffer(blob, dtype=np.uint8))
+    pos = len(blob)
+    has_icls = (np.asarray(cols["obj_flags"]) & 2) != 0
+    icls = np.where(has_icls, cols["obj_ingress_class"], np.uint64(0)).astype(np.uint64)
+    for name, refs in (("obj_ingress_class", icls), ("ann_key", cols["ann_key"]), ("ann_val", cols["ann_val"]), ("lbi_hostname", cols["lbi_hostname"]),
+                       ("port_proto", cols["port_proto"])):
+        refs = np.asarray(refs, dtype=np.uint64)
+        ln = _len(refs)
+        loc = np.concatenate([[0], np.cumsum(ln)])[:-1].astype(np.int64)  # where each string starts inside this column's piece
+        idx = np.repeat(_off(refs) - loc, ln) + np.arange(int(ln.sum()), dtype=np.int64)
+        pieces.append(slab[idx])
+        out[name] = (pos + loc).astype(np.uint64) | (ln.astype(np.uint64) << np.uint64(40))
+        pos += int(ln.sum())
+    out["slab"] = np.concatenate(pieces).astype(np.uint8) if pieces else np.zeros(0, dtype=np.uint8)
+    return out
+
+
+def _pad16(cols: dict) -> dict:
+    out = dict(cols)
+    s = np.asarray(cols["slab"], dtype=np.uint8)
+    out["slab"] = np.concatenate([s, np.zeros((-len(s)) % 16, dtype=np.uint8)])
+    return out
+
+
+class ColumnMirror:
+    """The object table after a sequence of deltas, as a column dict laid out like the engine's resident table."""
+
+    def __init__(self, o_cols: dict):
+        self.cur = {k: np.array(v, copy=True) for k, v in o_cols.items()}
+        self.slab_len = len(self.cur["slab"])
+        self.keys = row_keys(self.cur)
+        self.rows_of: dict = {}
+        for i, k in enumerate(self.keys):
+            self.rows_of.setdefault(k, []).append(i)
+
+    def apply(self, up: dict | None, deleted):
+        """up: upsert column dict (own slab) or None; deleted: [(kind, "ns/name")].  -> (upsert_row, deleted_row, moved_from)."""
+        n = len(self.keys)
+        src = {}  # new row -> ("c", current row) | ("u", upsert row), where not the identity
+        up_keys = row_keys(up) if up is not None and len(up["obj_kind"]) else []
+        del_row, moved, up_row = [], [], []
+        keys, rows_of = self.keys, self.rows_of
+
+        def lowest(k):
+            rs = rows_of.get(k)
+            return min(rs) if rs else GAR_NONE
+
+        for kind, name in deleted:
+            k = (int(kind), name.encode("utf-8", "surrogateescape") if isinstance(name, str) else name)
+            r = lowest(k)
+            del_row.append(r)
+            moved.append(GAR_NONE)
+            if r == GAR_NONE:
+                continue
+            last = n - 1
+            rows_of[k].remove(r)
+            if r != last:
+                lk = keys[last]
+                rows_of[lk].remove(last)
+                rows_of[lk].append(r)
+                keys[r] = lk
+                src[r] = src.pop(last, ("c", last))
+                moved[-1] = last
+            else:
+                src.pop(last, None)
+            keys.pop()
+            n -= 1
+        for u, k in enumerate(up_keys):
+            r = lowest(k)
+            if r == GAR_NONE:
+                r = n
+                n += 1
+                keys.append(k)
+                rows_of.setdefault(k, []).append(r)
+            src[r] = ("u", u)
+            up_row.append(r)
+        n_cur = len(self.cur["obj_kind"])
+        if up_keys:
+            both = tables.concat_cols(tables.OBJ_TABLES, ["obj", "ann", "lbi", "port"], [_pad16(self.cur), up])
+            self.slab_len = len(_pad16(self.cur)["slab"]) + len(up["slab"])
+        else:
+            both = self.cur
+        sel = np.arange(n, dtype=np.int64)
+        for r, (t, i) in src.items():
+            sel[r] = i if t == "c" else n_cur + i
+        self.cur = take_rows(both, sel)
+        self.cur["slab"] = np.asarray(both["slab"])
+        return np.array(up_row, dtype=np.uint32), np.array(del_row, dtype=np.uint32), np.array(moved, dtype=np.uint32)
+
+    def snapshot(self, a_cols: dict) -> "tables.Snapshot":
+        """A loadable snapshot of the mirrored object table with the given AWS tables."""
+        return tables.from_columns(self.cur, a_cols)
+
+
+def churn(mirror: ColumnMirror, rng: np.random.Generator, frac: float = 0.01, serial: int = 0):
+    """One informer-like batch over `frac` of the objects: updates that change decisions (another lbIngress hostname, another
+    route53-hostname annotation value, another listen-ports annotation value), 0.05 % adds with fresh keys, 0.05 % deletes.
+    -> (upsert column dict with its own slab, [(kind, "ns/name")] deleted keys)."""
+    cur = mirror.cur
+    n = len(cur["obj_kind"])
+    n_add = max(1, int(n * 0.0005))
+    n_del = max(1, int(n * 0.0005))
+    n_upd = max(1, int(n * frac) - n_add - n_del)
+    pick = rng.choice(n, size=min(n, n_upd + n_del), replace=False)
+    dels, upd = pick[:n_del], pick[n_del:]
+    adds = rng.choice(n, size=n_add, replace=False)
+    rows = np.concatenate([upd, adds])
+    U = take_rows(cur, rows)
+    slab = np.asarray(cur["slab"])
+    # the three kinds of decision-changing update, round robin over the updated rows
+    lb = np.asarray(cur["obj_lbi_begin"]).astype(np.int64)
+    with_lbi = np.flatnonzero(lb[1:] > lb[:-1])
+    ub = U["obj_lbi_begin"].astype(np.int64)
+    for j in range(0, len(upd), 3):
+        if ub[j + 1] > ub[j] and len(with_lbi):
+            U["lbi_hostname"][ub[j]] = cur["lbi_hostname"][lb[rng.choice(with_lbi)]]
+    ab = U["obj_ann_begin"].astype(np.int64)
+    for lit, phase in ((ANN_R53, 1), (ANN_LISTEN, 2)):
+        pool = np.asarray(cur["ann_val"])[key_is(np.asarray(cur["ann_key"]), slab, lit)]
+        if not len(pool):
+            continue
+        hit = key_is(U["ann_key"], slab, lit)
+        owner = np.searchsorted(ab, np.arange(len(hit)), side="right") - 1
+        sel = np.flatnonzero(hit & (owner < len(upd)) & (owner % 3 == phase))
+        if len(sel):
+            U["ann_val"][sel] = pool[rng.integers(0, len(pool), size=len(sel))]
+    keys = row_keys(U)
+    new_keys = [None] * len(upd) + [k[:k.index(b"/") + 1] + b"d%d-%d-" % (serial, i) + k[k.index(b"/") + 1:] for i, (_, k) in enumerate(keys[len(upd):])]
+    deleted = [(mirror.keys[r][0], mirror.keys[r][1].decode("utf-8", "surrogateescape")) for r in dels.tolist()]
+    return compact(U, new_keys), deleted
+
+
+def objects_struct(cols: dict):
+    """(Snapshot owning the buffers, its GarObjects) for an object column dict: the `upserts` of Engine.apply_objects."""
+    empty_actual = {c: np.zeros(0 if not isinstance(k, tuple) else 1, dtype=np.uint32 if isinstance(k, tuple) else tables._DT[k])
+                    for t, (_, cl) in tables.ACT_TABLES.items() for c, k in cl}
+    empty_actual["slab"] = np.zeros(0, dtype=np.uint8)
+    snap = tables.from_columns(cols, empty_actual)
+    return snap, snap.objects

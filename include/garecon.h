@@ -380,6 +380,46 @@ typedef struct gar_keyset {
 } gar_keyset;
 int gar_diff_keys(gar_engine *e, const gar_keyset *keys, gar_changeset *out);
 
+/* ---------------------------------------------------------------- object deltas: keeping the resident snapshot current
+   Informer events (add / update / delete of a Service or Ingress) applied to the loaded object table on the device, so that
+   gar_diff_keys (and gar_diff, gar_bindings_diff) see them without a reload.  The AWS tables are left as loaded.
+   A key is (kind, "ns/name").  Rules:
+     - a key appears at most once per delta, counting deletes and upserts together (the caller coalesces events, as the
+       workqueue does); otherwise GAR_E_INVALID;
+     - deletes run first, in the given order: the key's row (the lowest row at that moment if several rows carry the key;
+       a load may hold duplicates, an informer never does) is removed; unless it is the last row, the current last row moves
+       into it (moved_from).  n_objects decreases by one.  A key that is not present is a no-op (deleted_row = GAR_NONE);
+     - upserts run next, in the given order: a present key (lowest row) is replaced in place, an absent one appended as
+       row n_objects.
+   The table stays dense (object row order has no meaning: informer List order is unspecified), so every later call sees a
+   table exactly like the one a gar_snapshot_load of the same objects would give, with two exceptions that the change set
+   shows: tok_name / tok_region reference the resident object slab, where the strings of delta k sit at its slab_base.
+   The resident object slab is append-only: strings of replaced and deleted rows stay until the next gar_snapshot_load;
+   slab_len tells the caller when a reload is worth it.
+   Atomic: the upsert table passes the checks of gar_snapshot_load (string references inside its own slab, monotone CSRs,
+   kind / spec-type range, the ns/name layout rule) and the key rule above before anything resident changes; on
+   GAR_E_INVALID the snapshot is unchanged.  A CUDA error in the middle leaves no loaded snapshot: later deltas return
+   GAR_E_STATE and diffs fail until the next load.  GAR_E_STATE before any load, on an attached snapshot (gar_snapshot_attach_device), once gar_shard_route has run on
+   the loaded slice, and on a sharded sub-snapshot.  The call drops the recorded launch sequence of the full diff.  The
+   digests and indexes of the AWS tables stay prepared; the object side is rebuilt by the next diff. */
+typedef struct gar_object_delta {
+  const gar_objects *upserts;      /* added or updated objects: a complete table with its own slab, packed like a load's;
+                                      NULL or n_objects == 0: no upserts */
+  uint32_t n_deleted;
+  const uint8_t *deleted_kind;     /* [n_deleted] GAR_KIND_* */
+  const char *const *deleted_key;  /* [n_deleted] NUL-terminated "ns/name" (as in gar_keyset) */
+} gar_object_delta;
+typedef struct gar_delta_result {  /* arrays are caller-allocated */
+  uint32_t *upsert_row;            /* [upserts->n_objects] final row of each upserted object */
+  uint32_t *deleted_row;           /* [n_deleted] row the key had when it was removed; GAR_NONE if it was not in the cache */
+  uint32_t *moved_from;            /* [n_deleted] row whose object moved into deleted_row[k]; GAR_NONE if none moved */
+  uint32_t n_objects;              /* resident rows after the delta */
+  uint64_t slab_base;              /* offset of this delta's upsert slab inside the resident object slab (16-byte aligned);
+                                      0 when the delta has no upserts */
+  uint64_t slab_len;               /* resident object slab bytes after the delta, strings of replaced rows included */
+} gar_delta_result;
+int gar_snapshot_apply_objects(gar_engine *e, const gar_object_delta *d, gar_delta_result *out);
+
 /* ---------------------------------------------------------------- EndpointGroupBinding set-diff (SURVEY.md §8 row f3)
    The third controller's decisions (pkg/controller/endpointgroupbinding/reconcile.go:20-217): finalizer handling and the
    set difference between the load balancers of the referenced Service/Ingress and status.endpointIds.  Evaluated against
