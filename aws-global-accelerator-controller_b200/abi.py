@@ -124,6 +124,34 @@ class DeltaResult:
         self.n_objects, self.slab_base, self.slab_len = int(n_objects), int(slab_base), int(slab_len)
 
 
+class GarActualDelta(C.Structure):
+    _fields_ = [("rows", C.POINTER(GarActual)), ("lb_target", _u32p), ("acc_target", _u32p), ("zone_target", _u32p),
+                ("n_lb_deleted", C.c_uint32), ("lb_deleted", _u32p), ("n_acc_deleted", C.c_uint32), ("acc_deleted", _u32p)]
+
+
+ACTUAL_DELTA_SIZES = ("n_lbs", "n_accels", "n_tags", "n_listeners", "n_port_ranges", "n_egs", "n_endpoints", "n_records", "n_values")
+
+
+class GarActualDeltaResult(C.Structure):
+    _fields_ = [(k, C.c_uint32) for k in ACTUAL_DELTA_SIZES] + [("slab_base", C.c_uint64), ("slab_len", C.c_uint64)]
+
+
+class ActualDeltaResult(tuple):
+    """Outcome of one AWS delta (include/garecon.h gar_actual_delta_result): the table sizes after the delta, slab_base and
+    slab_len, by name or in that order."""
+    __slots__ = ()
+    FIELDS = ACTUAL_DELTA_SIZES + ("slab_base", "slab_len")
+
+    def __new__(cls, res: GarActualDeltaResult):
+        return super().__new__(cls, tuple(int(getattr(res, k)) for k in cls.FIELDS))
+
+    def __getattr__(self, name):
+        try:
+            return self[self.FIELDS.index(name)]
+        except ValueError:
+            raise AttributeError(name) from None
+
+
 EGB_DELETING, EGB_HAS_FINALIZERS, EGB_OBSERVED = 1, 2, 4
 (OP_EGB_ADD_FINALIZER, OP_EGB_REMOVE_FINALIZER, OP_EGB_REMOVE_ENDPOINT, OP_EGB_ADD_ENDPOINT, OP_EGB_UPDATE_WEIGHT, OP_EGB_UPDATE_STATUS) = range(11, 17)
 ST_REQUEUE_1S = 8
@@ -274,6 +302,8 @@ def load_library(path: os.PathLike | None = None) -> C.CDLL:
     lib.gar_bindings_diff.restype = C.c_int
     lib.gar_snapshot_apply_objects.argtypes = [C.c_void_p, C.POINTER(GarObjectDelta), C.POINTER(GarDeltaResult)]
     lib.gar_snapshot_apply_objects.restype = C.c_int
+    lib.gar_snapshot_apply_actual.argtypes = [C.c_void_p, C.POINTER(GarActualDelta), C.POINTER(GarActualDeltaResult)]
+    lib.gar_snapshot_apply_actual.restype = C.c_int
     lib.gar_shard_route.argtypes = [C.c_void_p, C.POINTER(GarShard), C.c_int, _u64p, _u64p]
     lib.gar_shard_route.restype = C.c_int
     lib.gar_shard_pack.argtypes = [C.c_void_p, C.c_void_p]
@@ -307,7 +337,7 @@ def load_library(path: os.PathLike | None = None) -> C.CDLL:
 
 EXPORTED_SYMBOLS = (
     "gar_engine_create", "gar_engine_destroy", "gar_snapshot_load", "gar_snapshot_attach_device", "gar_diff",
-    "gar_diff_device", "gar_diff_keys", "gar_bindings_diff", "gar_snapshot_apply_objects", "gar_shard_route", "gar_shard_pack", "gar_shard_unpack", "gar_shard_blob_bytes",
+    "gar_diff_device", "gar_diff_keys", "gar_bindings_diff", "gar_snapshot_apply_objects", "gar_snapshot_apply_actual", "gar_shard_route", "gar_shard_pack", "gar_shard_unpack", "gar_shard_blob_bytes",
     "gar_shard_arena", "gar_shard_open_peers", "gar_shard_pack_peers",
     "gar_changeset_free", "gar_last_error", "gar_version", "gar_algorithmic_bytes",
     "gar_last_stage_timings", "gar_last_counters",
@@ -383,6 +413,18 @@ class Engine:
         res = GarDeltaResult(up_row.ctypes.data_as(_u32p), del_row.ctypes.data_as(_u32p), moved.ctypes.data_as(_u32p), 0, 0, 0)
         self._check(self.lib.gar_snapshot_apply_objects(self._h, C.byref(d), C.byref(res)))
         return DeltaResult(up_row[:nu].copy(), del_row[:len(deleted)].copy(), moved[:len(deleted)].copy(), res.n_objects, res.slab_base, res.slab_len)
+
+    def apply_actual(self, rows: GarActual | None = None, lb_target=(), acc_target=(), zone_target=(), lb_deleted=(), acc_deleted=()) -> ActualDeltaResult:
+        """AWS delta against the loaded snapshot (include/garecon.h gar_snapshot_apply_actual).  `rows`: a GarActual of re-listed
+        load balancers, accelerators (whole subtrees) and zones (whole record lists), e.g. tables.pack([], actual).actual (its
+        buffers must stay alive for the call); *_target[k]: the resident row delta row k replaces (GAR_NONE: append; zones:
+        always a resident row); *_deleted: resident rows removed.  Order preserving."""
+        lt, at, zt, ld, ad = (np.ascontiguousarray(np.asarray(list(v), dtype=np.uint32).reshape(-1)) for v in (lb_target, acc_target, zone_target, lb_deleted, acc_deleted))
+        p = lambda a: a.ctypes.data_as(_u32p)  # noqa: E731  (the arrays stay alive until the call returns)
+        d = GarActualDelta(C.pointer(rows) if rows is not None else None, p(lt), p(at), p(zt), len(ld), p(ld), len(ad), p(ad))
+        res = GarActualDeltaResult()
+        self._check(self.lib.gar_snapshot_apply_actual(self._h, C.byref(d), C.byref(res)))
+        return ActualDeltaResult(res)
 
     def bindings_diff(self, bindings) -> ChangeSet:
         """EndpointGroupBinding set-diff against the loaded snapshot; `bindings` has a .struct (GarBindings)."""

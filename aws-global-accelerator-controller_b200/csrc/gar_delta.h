@@ -19,8 +19,16 @@
 //   void *delta_col(int c, size_t bytes);              // column c (DC_*) of the STANDBY object column set
 //   void delta_swap();                                 // the standby set becomes the resident one
 //   u8 *delta_slab(u64 keep, u64 need);                // resident object slab with >= need bytes, the first `keep` preserved
+//   void *delta_actual_col(int c, size_t bytes);       // the standby buffer of AWS column c (AC_*): not the resident one
+//   void delta_actual_swap(int c);                     // column c's standby buffer becomes the resident one
+//   u8 *delta_actual_slab(u64 keep, u64 need);         // the same as delta_slab, for the resident AWS slab
+//
+// AWS deltas (gar_snapshot_apply_actual, ActualSplicer below) re-lay only the AWS families a delta touches — load balancers;
+// accelerator -> tag / listener -> port range / listener -> endpoint group -> endpoint; zone -> record -> value — with one
+// generic step per parent -> child link, order preserving.  They drop the whole prepared state (the caller does).
 #pragma once
 
+#include <stddef.h>
 #include <string.h>
 
 #include <algorithm>
@@ -36,8 +44,23 @@ enum DeltaCol {
   DC_KIND, DC_SPEC, DC_FLAGS, DC_NS, DC_NAME, DC_ICLS, DC_ANN_B, DC_LBI_B, DC_PORT_B, DC_ANN_KEY, DC_ANN_VAL, DC_LBI_HOST, DC_PORT_NUM,
   DC_PORT_PROTO, DC_N
 };
-// staging buffers: the upsert columns (DS_UP + DC_*), keys, source map
-enum DeltaScratch { DS_UP = 0, DS_KEY_KIND = DC_N, DS_KEY_REF, DS_KEY_SLAB, DS_COUNTS, DS_OFFS, DS_ROWS, DS_PAIRS, DS_SRC, DS_TOTALS, DS_N };
+// AWS table columns, in gar_actual order (also the order in which gar_snapshot_load uploads them)
+enum ActualCol {
+  AC_LB_REGION, AC_LB_NAME, AC_LB_DNS, AC_LB_ARN, AC_LB_STATE, AC_ACC_NAME, AC_ACC_DNS, AC_ACC_ENABLED, AC_ACC_TAG_B, AC_ACC_LIS_B, AC_TAG_KEY,
+  AC_TAG_VAL, AC_LIS_PROTO, AC_LIS_PR_B, AC_LIS_EG_B, AC_PR_FROM, AC_EG_EP_B, AC_EP_ID, AC_ZONE_NAME, AC_ZONE_REC_B, AC_REC_NAME, AC_REC_TYPE,
+  AC_REC_ALIAS, AC_REC_ALIAS_DNS, AC_REC_VAL_B, AC_VAL_VALUE, AC_N
+};
+// AWS tables
+enum ActualTable { AT_LB, AT_ACC, AT_TAG, AT_LIS, AT_PR, AT_EG, AT_EP, AT_ZONE, AT_REC, AT_VAL, AT_N };
+// staging buffers: the upsert columns (DS_UP + DC_*), keys, source map; for AWS deltas the delta rows (DS_A_UP + AC_*), a
+// source map per table (DS_A_SRC + AT_*), the deleted / (new row, source) lists of the root tables and the zone-name check.
+// DS_A_COL + 2 * c (+ 1): the two buffers AWS column c alternates between, for a backend that keeps them with its staging
+// buffers (the host simulation; the CUDA engine has column sets of its own)
+enum DeltaScratch {
+  DS_UP = 0, DS_KEY_KIND = DC_N, DS_KEY_REF, DS_KEY_SLAB, DS_COUNTS, DS_OFFS, DS_ROWS, DS_PAIRS, DS_SRC, DS_TOTALS,
+  DS_A_UP, DS_A_SRC = DS_A_UP + AC_N, DS_A_DEL = DS_A_SRC + AT_N, DS_A_PAIRS = DS_A_DEL + AT_N, DS_A_ZTARGET = DS_A_PAIRS + AT_N, DS_A_ZREF,
+  DS_A_ZSLAB, DS_A_FLAG, DS_A_COL, DS_N = DS_A_COL + 2 * AC_N
+};
 
 constexpr u32 SRC_UPSERT = 0x80000000u;  // source map: row of the upsert batch (else a row of the resident table)
 
@@ -154,6 +177,120 @@ struct FDeltaChildren {
   }
 };
 
+// ------------------------------------------------------------------ AWS deltas: one generic step per parent -> child link
+// Every AWS table is re-laid by the same three functors.  A table's new rows come from a source map (resident row, or
+// SRC_UPSERT | row of the delta table); per CSR link the new begins are the children counts + one scan, and the children's
+// source map is written one warp per parent; then the child table is re-laid from that map, level by level.
+
+// survivors of an order-preserving delete: new row j <- resident row j + #{deleted rows before it}.  key[m] = d_m - m for
+// the deleted rows d ascending: the number of survivors ahead of the m-th deleted row, so the shift is #{m : key[m] <= j}
+struct FDeltaCompact {
+  const u32 *key;
+  u32 nd;
+  u32 *src;
+  GAR_HD void operator()(u32 j) const {
+    u32 lo = 0, hi = nd;
+    while (lo < hi) {
+      const u32 mid = (lo + hi) >> 1;
+      if (key[mid] <= j) lo = mid + 1;
+      else hi = mid;
+    }
+    src[j] = j + lo;
+  }
+};
+// new row i of a table: its fixed-width columns from its source row; string references of delta rows rebased by `base`
+struct DeltaGatherCol {
+  const u8 *r, *u;  // resident column, delta column
+  u8 *d;            // standby column
+  u32 width, str;
+};
+struct FDeltaGather {
+  const u32 *src;
+  u64 base;
+  u32 ncols;
+  DeltaGatherCol c[5];
+  GAR_HD void operator()(u32 i) const {
+    const u32 s = src[i], r = s & ~SRC_UPSERT;
+    const bool up = (s & SRC_UPSERT) != 0;
+    for (u32 k = 0; k < ncols; k++) {
+      const DeltaGatherCol &g = c[k];
+      const u8 *S = up ? g.u : g.r;
+      if (g.width == 1) g.d[i] = S[r];
+      else if (g.width == 4) ((u32 *)g.d)[i] = ((const u32 *)S)[r];
+      else ((u64 *)g.d)[i] = ((const u64 *)S)[r] + (up && g.str ? base : 0);  // the offset lives in the low bits of a gar_str
+    }
+  }
+};
+// child counts of new parent i (row n: the 0 that becomes the scan's total)
+struct FDeltaCsrCounts {
+  const u32 *src, *rb, *ub;  // parent source map, resident begins, delta begins
+  u32 n;
+  u32 *db;
+  GAR_HD void operator()(u32 i) const {
+    if (i == n) {
+      db[n] = 0;
+      return;
+    }
+    const u32 s = src[i], r = s & ~SRC_UPSERT;
+    const u32 *b = (s & SRC_UPSERT) ? ub : rb;
+    db[i] = b[r + 1] - b[r];
+  }
+};
+// the children's source map: 32 consecutive threads (one warp on the GPU) per new parent, striding over its children — a TXT
+// set of 10^5 values is not walked by one thread (DESIGN.md §4 "Skew")
+struct FDeltaCsrChildren {
+  const u32 *src, *rb, *ub, *db;
+  u32 *csrc;
+  GAR_HD void operator()(u32 t) const {
+    const u32 i = t >> 5, lane = t & 31u;
+    const u32 s = src[i], r = s & ~SRC_UPSERT, flag = s & SRC_UPSERT;
+    const u32 s0 = (flag ? ub : rb)[r], d0 = db[i], c = db[i + 1] - d0;
+    for (u32 k = lane; k < c; k += 32) csrc[d0 + k] = flag | (s0 + k);
+  }
+};
+// delta zone k must carry the name of resident zone target[k]
+struct FDeltaZoneName {
+  const u8 *rslab;
+  const gar_str *rname;
+  const u32 *target;
+  const u8 *dslab;
+  const gar_str *dname;
+  u32 *bad;
+  GAR_HD void operator()(u32 k) const {
+    if (!streq(mkstr(rslab, rname[target[k]]), mkstr(dslab, dname[k]))) *bad = 1;
+  }
+};
+
+// column layout of gar_actual: table, element width, gar_str or not, and the child table of a begin column (AT_N: none)
+struct ActualColInfo {
+  u8 table, width, str, child;
+  size_t field;
+};
+#define GAR_AC(t, w, s, ch, f) ActualColInfo{t, w, s, ch, offsetof(gar_actual, f)}
+static const ActualColInfo kActualCols[AC_N] = {
+    GAR_AC(AT_LB, 8, 1, AT_N, lb_region),          GAR_AC(AT_LB, 8, 1, AT_N, lb_name),          GAR_AC(AT_LB, 8, 1, AT_N, lb_dns),
+    GAR_AC(AT_LB, 8, 1, AT_N, lb_arn),             GAR_AC(AT_LB, 1, 0, AT_N, lb_state),         GAR_AC(AT_ACC, 8, 1, AT_N, acc_name),
+    GAR_AC(AT_ACC, 8, 1, AT_N, acc_dns),           GAR_AC(AT_ACC, 1, 0, AT_N, acc_enabled),     GAR_AC(AT_ACC, 4, 0, AT_TAG, acc_tag_begin),
+    GAR_AC(AT_ACC, 4, 0, AT_LIS, acc_lis_begin),   GAR_AC(AT_TAG, 8, 1, AT_N, tag_key),         GAR_AC(AT_TAG, 8, 1, AT_N, tag_val),
+    GAR_AC(AT_LIS, 1, 0, AT_N, lis_proto),         GAR_AC(AT_LIS, 4, 0, AT_PR, lis_pr_begin),   GAR_AC(AT_LIS, 4, 0, AT_EG, lis_eg_begin),
+    GAR_AC(AT_PR, 4, 0, AT_N, pr_from),            GAR_AC(AT_EG, 4, 0, AT_EP, eg_ep_begin),     GAR_AC(AT_EP, 8, 1, AT_N, ep_id),
+    GAR_AC(AT_ZONE, 8, 1, AT_N, zone_name),        GAR_AC(AT_ZONE, 4, 0, AT_REC, zone_rec_begin), GAR_AC(AT_REC, 8, 1, AT_N, rec_name),
+    GAR_AC(AT_REC, 1, 0, AT_N, rec_type),          GAR_AC(AT_REC, 1, 0, AT_N, rec_has_alias),   GAR_AC(AT_REC, 8, 1, AT_N, rec_alias_dns),
+    GAR_AC(AT_REC, 4, 0, AT_VAL, rec_val_begin),   GAR_AC(AT_VAL, 8, 1, AT_N, val_value)};
+#undef GAR_AC
+static const size_t kActualRows[AT_N] = {offsetof(gar_actual, n_lbs),         offsetof(gar_actual, n_accels), offsetof(gar_actual, n_tags),
+                                         offsetof(gar_actual, n_listeners),   offsetof(gar_actual, n_port_ranges), offsetof(gar_actual, n_egs),
+                                         offsetof(gar_actual, n_endpoints),   offsetof(gar_actual, n_zones),  offsetof(gar_actual, n_records),
+                                         offsetof(gar_actual, n_values)};
+static const char *const kActualColName[AC_N] = {
+    "lb_region", "lb_name", "lb_dns", "lb_arn", "lb_state", "acc_name", "acc_dns", "acc_enabled", "acc_tag_begin", "acc_lis_begin", "tag_key", "tag_val", "lis_proto",
+    "lis_pr_begin", "lis_eg_begin", "pr_from", "eg_ep_begin", "ep_id", "zone_name", "zone_rec_begin", "rec_name", "rec_type", "rec_has_alias", "rec_alias_dns",
+    "rec_val_begin", "val_value"};
+inline const void *&actual_col(gar_actual &a, int c) { return *(const void **)((char *)&a + kActualCols[c].field); }
+inline const void *actual_col(const gar_actual &a, int c) { return *(const void *const *)((const char *)&a + kActualCols[c].field); }
+inline u32 &actual_rows(gar_actual &a, int t) { return *(u32 *)((char *)&a + kActualRows[t]); }
+inline u32 actual_rows(const gar_actual &a, int t) { return *(const u32 *)((const char *)&a + kActualRows[t]); }
+
 // ------------------------------------------------------------------ host-side checks of the (small) upsert batch
 
 // the checks gar_snapshot_load runs on the device, for a table the host holds; "" = valid
@@ -188,6 +325,41 @@ inline std::string delta_check_upserts(const gar_objects &o) {
     if (!str_ok(o.lbi_hostname[k])) return "upserts: lbi_hostname: string reference outside the slab";
   for (u32 k = 0; k < o.n_ports; k++)
     if (!str_ok(o.port_proto[k])) return "upserts: port_proto: string reference outside the slab";
+  return "";
+}
+
+// the checks gar_snapshot_load runs on an actual table, for the rows of an AWS delta; "" = valid
+inline std::string delta_check_actual(const gar_actual &a) {
+  if (a.slab_len && !a.slab) return "rows: NULL slab";
+  for (int c = 0; c < AC_N; c++) {
+    const ActualColInfo &ci = kActualCols[c];
+    const u32 n = actual_rows(a, ci.table);
+    const void *col = actual_col(a, c);
+    const std::string name = std::string("rows: ") + kActualColName[c];
+    if (ci.child != AT_N) {
+      if (!col) return name + " is NULL";
+      const u32 *b = (const u32 *)col;
+      bool ok = b[0] == 0 && b[n] == actual_rows(a, ci.child);
+      for (u32 i = 0; ok && i < n; i++) ok = b[i + 1] >= b[i];
+      if (!ok) return name + ": CSR is not monotone, does not start at 0 or does not end at the child count";
+      continue;
+    }
+    if (!n) continue;
+    if (!col) return name + " is NULL";
+    if (ci.str) {
+      const gar_str *s = (const gar_str *)col;
+      for (u32 i = 0; i < n; i++)
+        if (GAR_STR_OFF(s[i]) + GAR_STR_LEN(s[i]) > a.slab_len) return name + ": string reference outside the slab";
+    }
+  }
+  auto enum_ok = [](const u8 *col, u32 n, u32 max_value) {
+    for (u32 i = 0; i < n; i++)
+      if (col[i] > max_value) return false;
+    return true;
+  };
+  if (!enum_ok(a.lb_state, a.n_lbs, GAR_LB_FAILED)) return "rows: lb_state out of range";
+  if (!enum_ok(a.lis_proto, a.n_listeners, GAR_PROTO_UDP)) return "rows: lis_proto out of range";
+  if (!enum_ok(a.rec_type, a.n_records, GAR_RR_AAAA)) return "rows: rec_type out of range";
   return "";
 }
 
@@ -411,5 +583,198 @@ struct Splicer {
   int invalid(const char *msg) {
     error = msg;
     return GAR_E_INVALID;
+  }
+};
+
+// ------------------------------------------------------------------ the AWS-delta driver
+// The order-preserving splice of include/garecon.h "AWS deltas".  The host checks the (small) delta and turns the targets
+// into a source map of each root table (LBs, accelerators, zones); only the families a delta touches are then re-laid into
+// standby columns by relayout(), level by level.  Nothing resident changes before the last level is written: the standby
+// columns become the resident ones at the end (delta_actual_swap).  The caller drops the pipeline's prepared state.
+template <class B>
+struct ActualSplicer {
+  B &be;
+  DevTables &T;  // the resident tables: T.a is replaced by a splice
+  std::string error;
+  gar_actual R{}, U{}, N{};  // resident table, delta rows (device copies), the table being built
+  u64 base = 0;
+  bool written[AC_N] = {};
+
+  // GAR_OK, GAR_E_INVALID (error says why; nothing changed) or another gar_rc
+  int apply(const gar_actual_delta &d, gar_actual_delta_result &out) {
+    static const u32 kZero[1] = {0};
+    gar_actual no_rows{};  // an empty table: every CSR is {0}
+    for (int c = 0; c < AC_N; c++)
+      if (kActualCols[c].child != AT_N) actual_col(no_rows, c) = kZero;
+    const gar_actual &H = d.rows ? *d.rows : no_rows;
+    R = T.a;
+    error = delta_check_actual(H);
+    if (!error.empty()) return GAR_E_INVALID;
+    if ((H.n_lbs && !d.lb_target) || (H.n_accels && !d.acc_target) || (H.n_zones && !d.zone_target) || (d.n_lb_deleted && !d.lb_deleted) ||
+        (d.n_acc_deleted && !d.acc_deleted))
+      return invalid("NULL target or deleted-row array");
+    std::vector<u32> lb_key, lb_pairs, acc_key, acc_pairs, zone_pairs;
+    u32 n_lbs = 0, n_accels = 0;
+    if (!plan("load balancer", R.n_lbs, H.n_lbs, d.lb_target, d.n_lb_deleted, d.lb_deleted, lb_key, lb_pairs, n_lbs)) return GAR_E_INVALID;
+    if (!plan("accelerator", R.n_accels, H.n_accels, d.acc_target, d.n_acc_deleted, d.acc_deleted, acc_key, acc_pairs, n_accels)) return GAR_E_INVALID;
+    if (n_accels >= (1u << 27)) return invalid("too many accelerators for one snapshot");
+    {
+      std::unordered_set<u32> seen;
+      for (u32 k = 0; k < H.n_zones; k++) {
+        const u32 z = d.zone_target[k];
+        if (z >= R.n_zones) return invalid("zone_target out of range (adding hosted zones is a reload)");
+        if (!seen.insert(z).second) return invalid("a zone appears twice in zone_target");
+        zone_pairs.push_back(z);
+        zone_pairs.push_back(SRC_UPSERT | k);
+      }
+    }
+    const bool has_rows = H.n_lbs || H.n_accels || H.n_zones;  // (a table without them has no children: its CSRs end at 0)
+    base = has_rows ? (R.slab_len + 15) & ~(u64)15 : 0;
+    if (has_rows && base + H.slab_len + GAR_SLAB_PAD >= (1ull << GAR_STR_OFF_BITS)) return invalid("the resident AWS slab would outgrow 2^40 bytes: reload");
+    if (H.n_zones && !zone_names_match(H, d.zone_target)) return invalid("a delta zone's zone_name differs from the name of the resident zone it replaces");
+    N = R;
+    const bool lbs = H.n_lbs || d.n_lb_deleted, accs = H.n_accels || d.n_acc_deleted;
+    if (lbs || accs || H.n_zones) {
+      // the delta rows on the device; their strings behind the resident ones
+      U = H;
+      for (int c = 0; c < AC_N; c++) {
+        const ActualColInfo &ci = kActualCols[c];
+        const size_t n = (size_t)actual_rows(H, ci.table) + (ci.child != AT_N ? 1 : 0);
+        actual_col(U, c) = up(DS_A_UP + c, actual_col(H, c), n * ci.width);
+      }
+      if (has_rows) {
+        u8 *slab = be.delta_actual_slab(R.slab_len, base + H.slab_len + GAR_SLAB_PAD);
+        static const u8 kZeros[GAR_SLAB_PAD] = {};
+        if (H.slab_len) be.upload(slab + base, H.slab, H.slab_len);
+        be.upload(slab + base + H.slab_len, kZeros, GAR_SLAB_PAD);
+        T.a.slab = N.slab = slab;  // the resident bytes moved with a grown slab; slab_len changes only with the rest
+        N.slab_len = base + H.slab_len;
+      }
+      int rc = GAR_OK;
+      if (lbs) rc = relayout(AT_LB, root_map(AT_LB, n_lbs, lb_key, lb_pairs), n_lbs);
+      if (rc == GAR_OK && accs) rc = relayout(AT_ACC, root_map(AT_ACC, n_accels, acc_key, acc_pairs), n_accels);
+      if (rc == GAR_OK && H.n_zones) rc = relayout(AT_ZONE, root_map(AT_ZONE, R.n_zones, {}, zone_pairs), R.n_zones);
+      if (rc != GAR_OK) return rc;
+      for (int c = 0; c < AC_N; c++)
+        if (written[c]) be.delta_actual_swap(c);
+      T.a = N;
+    }
+    out.n_lbs = T.a.n_lbs;
+    out.n_accels = T.a.n_accels;
+    out.n_tags = T.a.n_tags;
+    out.n_listeners = T.a.n_listeners;
+    out.n_port_ranges = T.a.n_port_ranges;
+    out.n_egs = T.a.n_egs;
+    out.n_endpoints = T.a.n_endpoints;
+    out.n_records = T.a.n_records;
+    out.n_values = T.a.n_values;
+    out.slab_base = base;
+    out.slab_len = T.a.slab_len;
+    return GAR_OK;
+  }
+
+ private:
+  int invalid(const std::string &msg) {
+    error = msg;
+    return GAR_E_INVALID;
+  }
+  const void *up(int k, const void *host, size_t bytes) {
+    void *p = be.delta_scratch(k, bytes + GAR_SLAB_PAD + 16);
+    if (bytes) be.upload(p, host, bytes);
+    return p;
+  }
+  void *standby(int c, size_t bytes) {
+    written[c] = true;
+    void *p = be.delta_actual_col(c, bytes + 16);
+    actual_col(N, c) = p;
+    return p;
+  }
+
+  // targets and deletes of a root table with order-preserving deletes: the compaction keys (deleted rows ascending, minus
+  // their rank) and the (new row, source) pairs of the replaced and appended rows
+  bool plan(const char *what, u32 n, u32 nu, const u32 *target, u32 nd, const u32 *deleted, std::vector<u32> &key, std::vector<u32> &pairs, u32 &n_new) {
+    std::unordered_set<u32> seen;
+    for (u32 k = 0; k < nd + nu; k++) {
+      const u32 r = k < nd ? deleted[k] : target[k - nd];
+      if (k >= nd && r == GAR_NONE) continue;
+      if (r >= n) {
+        invalid(std::string(what) + " row out of range");
+        return false;
+      }
+      if (!seen.insert(r).second) {
+        invalid(std::string("a resident ") + what + " row appears twice among the targets and deleted rows");
+        return false;
+      }
+    }
+    key.assign(deleted, deleted + nd);
+    std::sort(key.begin(), key.end());
+    const u32 survivors = n - nd;
+    u32 appended = 0;
+    for (u32 k = 0; k < nu; k++) {
+      const u32 r = target[k];
+      pairs.push_back(r == GAR_NONE ? survivors + appended++ : r - (u32)(std::lower_bound(key.begin(), key.end(), r) - key.begin()));
+      pairs.push_back(SRC_UPSERT | k);
+    }
+    for (u32 m = 0; m < nd; m++) key[m] -= m;
+    n_new = survivors + appended;
+    return true;
+  }
+
+  bool zone_names_match(const gar_actual &H, const u32 *target) {
+    std::vector<u8> zslab;
+    std::vector<gar_str> zref(H.n_zones);
+    for (u32 k = 0; k < H.n_zones; k++) {
+      const u32 len = GAR_STR_LEN(H.zone_name[k]);
+      const u8 *p = H.slab + GAR_STR_OFF(H.zone_name[k]);
+      zref[k] = GAR_STR(zslab.size(), len);
+      zslab.insert(zslab.end(), p, p + len);
+    }
+    zslab.resize(zslab.size() + GAR_SLAB_PAD, 0);
+    const u32 zero = 0;
+    u32 *bad = (u32 *)up(DS_A_FLAG, &zero, 4);
+    be.for_each("delta_zone_names", H.n_zones,
+                FDeltaZoneName{R.slab, R.zone_name, (const u32 *)up(DS_A_ZTARGET, target, 4 * (size_t)H.n_zones), (const u8 *)up(DS_A_ZSLAB, zslab.data(), zslab.size()),
+                               (const gar_str *)up(DS_A_ZREF, zref.data(), 8 * (size_t)H.n_zones), bad});
+    u32 flag = 0;
+    be.download(&flag, bad, 4);
+    return flag == 0;
+  }
+
+  // source map of a root table: identity or the survivors of the deletes, then the replaced / appended rows
+  const u32 *root_map(int t, u32 n, const std::vector<u32> &key, const std::vector<u32> &pairs) {
+    u32 *src = (u32 *)be.delta_scratch(DS_A_SRC + t, 4 * (size_t)(n + 1));
+    if (n && key.empty()) be.for_each("delta_source_map", n, FDeltaIdentity{src});
+    if (n && !key.empty()) be.for_each("delta_source_map", n, FDeltaCompact{(const u32 *)up(DS_A_DEL + t, key.data(), 4 * key.size()), (u32)key.size(), src});
+    if (!pairs.empty()) be.for_each("delta_source_map", (u32)(pairs.size() / 2), FDeltaScatter{(const u32 *)up(DS_A_PAIRS + t, pairs.data(), 4 * pairs.size()), src});
+    return src;
+  }
+
+  // table t gets the n rows src names: its fixed-width columns are gathered, and each CSR link to a child table yields the new
+  // begins (counts + scan) and the children's source map, from which the child table is re-laid in turn
+  int relayout(int t, const u32 *src, u32 n) {
+    actual_rows(N, t) = n;
+    FDeltaGather g{src, base, 0, {}};
+    for (int c = 0; c < AC_N; c++) {
+      const ActualColInfo &ci = kActualCols[c];
+      if (ci.table != t || ci.child != AT_N || c == AC_ZONE_NAME) continue;  // zone rows never move: only their record lists change
+      g.c[g.ncols++] = DeltaGatherCol{(const u8 *)actual_col(R, c), (const u8 *)actual_col(U, c), (u8 *)standby(c, (size_t)n * ci.width), ci.width, ci.str};
+    }
+    if (g.ncols && n) be.for_each("delta_gather", n, g);
+    for (int c = 0; c < AC_N; c++) {
+      const ActualColInfo &ci = kActualCols[c];
+      if (ci.table != t || ci.child == AT_N) continue;
+      const u32 *rb = (const u32 *)actual_col(R, c), *ub = (const u32 *)actual_col(U, c);
+      u32 *db = (u32 *)standby(c, 4 * (size_t)(n + 1));
+      be.for_each("delta_csr_counts", n + 1, FDeltaCsrCounts{src, rb, ub, n, db});
+      be.exclusive_scan(db, n + 1);
+      u32 nc = 0;
+      be.download(&nc, db + n, 4);
+      if (nc >= (1u << 27)) return invalid(std::string(kActualColName[c]) + ": too many rows for one snapshot");
+      u32 *csrc = (u32 *)be.delta_scratch(DS_A_SRC + ci.child, 4 * (size_t)(nc + 1));
+      if (n) be.for_each("delta_csr_children", n * 32, FDeltaCsrChildren{src, rb, ub, db, csrc});
+      const int rc = relayout(ci.child, csrc, nc);
+      if (rc != GAR_OK) return rc;
+    }
+    return GAR_OK;
   }
 };

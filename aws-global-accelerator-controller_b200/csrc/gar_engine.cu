@@ -865,8 +865,16 @@ struct gar_engine {
   void *delta_scratch(int k, size_t bytes) { return dev_ensure(dscratch[k], bytes); }
   void *delta_col(int c, size_t bytes) { return dev_ensure(o_set == 0 ? dset[c] : in[c], bytes); }
   void delta_swap() { o_set ^= 1; }
-  u8 *delta_slab(u64 keep, u64 need) {
-    DBuf &b = in[DC_N];
+  u8 *delta_slab(u64 keep, u64 need) { return grow_slab(in[DC_N], keep, need); }
+  // ---- AWS deltas: column c of the AWS tables lives in in[DC_N + 1 + c] (as gar_snapshot_load left it) or in aset[c]
+  // (a_alt[c]); only the columns a delta re-lays alternate.  The AWS slab stays in in[DC_N + 1 + AC_N].
+  DBuf aset[AC_N];
+  bool a_alt[AC_N] = {};
+  void *delta_actual_col(int c, size_t bytes) { return dev_ensure(a_alt[c] ? in[DC_N + 1 + c] : aset[c], bytes); }
+  void delta_actual_swap(int c) { a_alt[c] = !a_alt[c]; }
+  u8 *delta_actual_slab(u64 keep, u64 need) { return grow_slab(in[DC_N + 1 + AC_N], keep, need); }
+  // an append-only slab with room for `need` bytes, the first `keep` preserved
+  u8 *grow_slab(DBuf &b, u64 keep, u64 need) {
     if (b.cap < need + 16) {
       graph_drop();
       size_t want = (size_t)(need + need / 2 + 256) & ~(size_t)255;
@@ -1012,7 +1020,8 @@ static void do_load(gar_engine *e, const gar_objects *o, const gar_actual *a) {
   validate_pointers(o, a);  // NULL checks before anything is copied; the contents are checked on the device, below
   CK(cudaSetDevice(e->device));
   e->in_used = 0;
-  e->o_set = 0;  // the object columns go to in[DC_*] again
+  e->o_set = 0;  // the object columns go to in[DC_*] again, the AWS columns to in[DC_N + 1 + AC_*]
+  for (bool &alt : e->a_alt) alt = false;
   DevTables &T = e->T;
   CK(cudaEventRecord(e->ev[0], e->stream));
   T.o = *o;
@@ -1112,6 +1121,36 @@ static void do_apply(gar_engine *e, const gar_object_delta *d, gar_delta_result 
     if (rc == GAR_E_INVALID) throw InvalidError{S.error};
     if (rc != GAR_OK) throw StateError{"the object delta could not be applied"};
     e->slice = e->T;
+    e->input_bytes = table_bytes(&e->T.o, &e->T.a);  // counts and slab lengths only
+  } catch (const CudaError &) {
+    e->loaded = false;  // the splice may have stopped half-way: no snapshot until the next load
+    delete e->pipe;
+    e->pipe = nullptr;
+    throw;
+  }
+}
+
+static void do_apply_actual(gar_engine *e, const gar_actual_delta *d, gar_actual_delta_result *out) {
+  if (!e->loaded) throw StateError{"no snapshot loaded"};
+  if (e->attached) throw StateError{"AWS deltas need a snapshot the engine owns: an attached (device) snapshot cannot be changed"};
+  if (e->shard_home || e->shard_round != 0) throw StateError{"AWS deltas are not available in sharded mode"};
+  CK(cudaSetDevice(e->device));
+  e->graph_drop();
+  e->marks.clear();
+  e->events_used = 0;
+  e->stage_depth = 0;
+  try {
+    ActualSplicer<gar_engine> S{*e, e->T};
+    const int rc = S.apply(*d, *out);
+    CK(cudaStreamSynchronize(e->stream));
+    CK(cudaGetLastError());
+    e->slice = e->T;  // the slab may have moved even when the delta was refused (its resident bytes unchanged)
+    if (e->pipe) {
+      e->pipe->T = e->T;
+      if (rc == GAR_OK) e->pipe->prepared = false;  // the next diff prepares the snapshot as the first one after a load
+    }
+    if (rc == GAR_E_INVALID) throw InvalidError{S.error};
+    if (rc != GAR_OK) throw StateError{"the AWS delta could not be applied"};
     e->input_bytes = table_bytes(&e->T.o, &e->T.a);  // counts and slab lengths only
   } catch (const CudaError &) {
     e->loaded = false;  // the splice may have stopped half-way: no snapshot until the next load
@@ -1401,6 +1440,7 @@ void gar_engine_destroy(gar_engine *e) {
   for (auto &b : e->d_egb) cudaFree(b.p);
   for (auto &b : e->dset) cudaFree(b.p);
   for (auto &b : e->dscratch) cudaFree(b.p);
+  for (auto &b : e->aset) cudaFree(b.p);
   cudaFree(e->d_valid.p);
   for (int k = 0; k < 2; k++) {
     if (e->dl_pin[k].p) cudaFreeHost(e->dl_pin[k].p);
@@ -1471,6 +1511,11 @@ int gar_bindings_diff(gar_engine *e, const gar_bindings *bindings, gar_changeset
 int gar_snapshot_apply_objects(gar_engine *e, const gar_object_delta *d, gar_delta_result *out) {
   if (!d || !out) return GAR_E_INVALID;
   return guarded(e, [&] { do_apply(e, d, out); });
+}
+
+int gar_snapshot_apply_actual(gar_engine *e, const gar_actual_delta *d, gar_actual_delta_result *out) {
+  if (!d || !out) return GAR_E_INVALID;
+  return guarded(e, [&] { do_apply_actual(e, d, out); });
 }
 
 int gar_shard_route(gar_engine *e, const gar_shard *shard, int round, uint64_t *meta, uint64_t *send_bytes) {

@@ -209,6 +209,185 @@ def churn(mirror: ColumnMirror, rng: np.random.Generator, frac: float = 0.01, se
     return compact(U, new_keys), deleted
 
 
+# ------------------------------------------------------------------ AWS deltas (gar_snapshot_apply_actual)
+
+def take_tree(cols: dict, table: str, rows, out: dict | None = None) -> dict:
+    """Rows `rows` (in that order) of an AWS table of an actual column dict, with every table below it (children follow their
+    parents, as a load lays them out); string references unchanged."""
+    out = {} if out is None else out
+    rows = np.asarray(rows, dtype=np.int64)
+    for name, kind in tables.ACT_TABLES[table][1]:
+        if isinstance(kind, tuple):
+            b = np.asarray(cols[name]).astype(np.int64)
+            cnt = b[rows + 1] - b[rows]
+            nb = np.concatenate([[0], np.cumsum(cnt)]).astype(np.int64)
+            idx = np.repeat(b[rows] - nb[:-1], cnt) + np.arange(nb[-1], dtype=np.int64)
+            out[name] = nb.astype(np.uint32)
+            take_tree(cols, kind[1], idx, out)
+        else:
+            out[name] = np.asarray(cols[name])[rows]
+    return out
+
+
+def compact_actual(cols: dict) -> dict:
+    """An actual column dict with a slab of its own that holds exactly the strings it references."""
+    slab = np.asarray(cols["slab"])
+    out = {k: np.array(v, copy=True) for k, v in cols.items() if k != "slab"}
+    pieces, pos = [], 0
+    for t, (_, cl) in tables.ACT_TABLES.items():
+        for name, kind in cl:
+            if kind != "str":
+                continue
+            refs = np.asarray(cols[name], dtype=np.uint64)
+            if name == "rec_alias_dns":
+                refs = np.where(np.asarray(cols["rec_has_alias"]) != 0, refs, np.uint64(0)).astype(np.uint64)
+            ln = _len(refs)
+            loc = np.concatenate([[0], np.cumsum(ln)])[:-1].astype(np.int64)
+            idx = np.repeat(_off(refs) - loc, ln) + np.arange(int(ln.sum()), dtype=np.int64)
+            pieces.append(slab[idx])
+            out[name] = (pos + loc).astype(np.uint64) | (ln.astype(np.uint64) << np.uint64(40))
+            pos += int(ln.sum())
+    out["slab"] = np.concatenate(pieces).astype(np.uint8) if pieces else np.zeros(0, dtype=np.uint8)
+    return out
+
+
+def actual_rows(cols: dict, lb_rows=(), acc_rows=(), zone_rows=()) -> dict:
+    """A small actual table (the `rows` of an AWS delta, before compact_actual): load balancers `lb_rows`, accelerators
+    `acc_rows` with their subtrees and zones `zone_rows` with their record lists, taken from `cols`."""
+    out = take_tree(cols, "lb", lb_rows)
+    take_tree(cols, "acc", acc_rows, out)
+    take_tree(cols, "zone", zone_rows, out)
+    out["slab"] = cols["slab"]
+    return out
+
+
+class ActualMirror:
+    """The AWS tables after a sequence of AWS deltas, as a column dict laid out like the engine's resident tables (the rules of
+    include/garecon.h "AWS deltas"): order preserving, each delta's slab appended at a 16-byte aligned slab_base."""
+
+    def __init__(self, a_cols: dict):
+        self.cur = {k: np.array(v, copy=True) for k, v in a_cols.items()}
+        self.slab_len = len(self.cur["slab"])
+
+    def sizes(self) -> dict:
+        return {nf: len(self.cur[cl[0][0]]) - (1 if isinstance(cl[0][1], tuple) else 0) for t, (nf, cl) in tables.ACT_TABLES.items()}
+
+    def apply(self, rows: dict | None, lb_target=(), acc_target=(), zone_target=(), lb_deleted=(), acc_deleted=()) -> dict:
+        """rows: actual column dict with its own slab, or None.  -> the result of the delta: table sizes, slab_base, slab_len."""
+        cur = self.cur
+        n_rows = {t: len(rows[cl[0][0]]) - (1 if isinstance(cl[0][1], tuple) else 0) for t, (_, cl) in tables.ACT_TABLES.items()} if rows else {}
+        has_rows = bool(rows) and (n_rows["lb"] + n_rows["acc"] + n_rows["zone"]) > 0
+        base = 0
+        both = cur
+        if has_rows:
+            padded = _pad16(cur)
+            base = len(padded["slab"])
+            both = tables.concat_cols(tables.ACT_TABLES, ["lb", "acc", "tag", "lis", "pr", "eg", "ep", "rec", "val"], [padded, rows])
+            both["zone_name"] = cur["zone_name"]
+            both["zone_rec_begin"] = cur["zone_rec_begin"]
+        new = {}
+
+        def root(table, nf, target, deleted):
+            n = len(cur[nf])
+            gone = set(int(r) for r in deleted)
+            repl = {int(r): k for k, r in enumerate(target) if int(r) != GAR_NONE}
+            sel = [n + repl[r] if r in repl else r for r in range(n) if r not in gone]
+            sel += [n + k for k, r in enumerate(target) if int(r) == GAR_NONE]
+            take_tree(both, table, np.asarray(sel, dtype=np.int64), new)
+
+        root("lb", "lb_state", lb_target, lb_deleted)
+        root("acc", "acc_enabled", acc_target, acc_deleted)
+        zb = np.asarray(cur["zone_rec_begin"]).astype(np.int64)
+        zrepl = {int(z): k for k, z in enumerate(zone_target)}
+        n_rec = int(zb[-1])
+        rec_sel = []
+        if zrepl:
+            rb = np.asarray(rows["zone_rec_begin"]).astype(np.int64)
+        for z in range(len(zb) - 1):
+            if z in zrepl:
+                k = zrepl[z]
+                rec_sel.append(np.arange(rb[k], rb[k + 1]) + n_rec)
+            else:
+                rec_sel.append(np.arange(zb[z], zb[z + 1]))
+        cnt = [len(s) for s in rec_sel]
+        new["zone_name"] = cur["zone_name"]
+        new["zone_rec_begin"] = np.concatenate([[0], np.cumsum(cnt)]).astype(np.uint32)
+        take_tree(both, "rec", np.concatenate(rec_sel).astype(np.int64) if rec_sel else np.zeros(0, dtype=np.int64), new)
+        new["slab"] = np.asarray(both["slab"])
+        self.cur = new
+        self.slab_len = len(new["slab"])
+        out = dict(self.sizes())
+        out.pop("n_zones")
+        out["slab_base"] = base
+        out["slab_len"] = self.slab_len
+        return out
+
+    def snapshot(self, o_cols: dict) -> "tables.Snapshot":
+        """A loadable snapshot of the given object table with the mirrored AWS tables."""
+        return tables.from_columns(o_cols, self.cur)
+
+
+def aws_churn(mirror: ActualMirror, rng: np.random.Generator, frac: float = 0.01, max_zones: int = 4):
+    """One re-list batch over `frac` of the AWS rows, like the lists a worker re-issues after executing a batch: load balancer
+    state flips plus a few appended (duplicate (region, name)) and deleted LBs; accelerator subtrees rewritten (a tag value,
+    listener ports, endpoints), a few accelerators appended (copies) and deleted; the record lists of up to `max_zones` zones
+    replaced (a record dropped, another repeated).  -> keyword arguments of Engine.apply_actual / ActualMirror.apply, with
+    rows = a compact actual column dict."""
+    cur = mirror.cur
+    n_lb, n_acc, n_zone = len(cur["lb_state"]), len(cur["acc_enabled"]), len(cur["zone_name"])
+
+    def split(n, k_change, k_del):
+        pick = rng.choice(n, size=min(n, k_change + k_del), replace=False) if n else np.zeros(0, dtype=np.int64)
+        return np.sort(pick[k_del:]), np.sort(pick[:k_del])
+
+    lb_upd, lb_del = split(n_lb, max(1, int(n_lb * frac)), max(1, int(n_lb * frac / 20)) if n_lb > 2 else 0)
+    lb_add = rng.choice(n_lb, size=max(1, int(n_lb * frac / 20)), replace=True) if n_lb else np.zeros(0, dtype=np.int64)
+    acc_upd, acc_del = split(n_acc, max(1, int(n_acc * frac)), max(1, int(n_acc * frac / 20)) if n_acc > 2 else 0)
+    acc_add = rng.choice(n_acc, size=max(1, int(n_acc * frac / 20)), replace=True) if n_acc else np.zeros(0, dtype=np.int64)
+    zones = np.sort(rng.choice(n_zone, size=min(n_zone, max_zones), replace=False)) if n_zone else np.zeros(0, dtype=np.int64)
+    rows = actual_rows(cur, np.concatenate([lb_upd, lb_add]), np.concatenate([acc_upd, acc_add]), zones)
+    # load balancers: state flips on the re-described rows, another row's DNS name on the appended copies
+    st = rows["lb_state"]
+    st[:len(lb_upd)] = np.where(st[:len(lb_upd)] == 0, 1, 0)
+    if len(lb_add):
+        rows["lb_dns"][len(lb_upd):] = cur["lb_dns"][rng.integers(0, n_lb, size=len(lb_add))]
+    # accelerator subtrees: a tag value, listener ports and endpoints taken from elsewhere in the batch
+    if len(rows["tag_val"]):
+        t = rng.random(len(rows["tag_val"])) < 0.2
+        rows["tag_val"][t] = rows["tag_val"][rng.integers(0, len(rows["tag_val"]), size=int(t.sum()))]
+    if len(rows["pr_from"]):
+        p = rng.random(len(rows["pr_from"])) < 0.3
+        rows["pr_from"][p] = rng.choice(np.array([80, 443, 8080, 53], dtype=np.int32), size=int(p.sum()))
+    if len(rows["ep_id"]):
+        rows["ep_id"] = rows["ep_id"][rng.permutation(len(rows["ep_id"]))]
+    # record lists: per zone, one record dropped and another one repeated
+    zb = rows["zone_rec_begin"].astype(np.int64)
+    keep = []
+    for k in range(len(zones)):
+        recs = list(range(zb[k], zb[k + 1]))
+        if recs and rng.random() < 0.7:
+            recs.pop(int(rng.integers(0, len(recs))))
+        if recs and rng.random() < 0.5:
+            recs.append(recs[int(rng.integers(0, len(recs)))])
+        keep.append(recs)
+    rec_rows = take_tree(rows, "rec", np.asarray([r for rs in keep for r in rs], dtype=np.int64))
+    rows.update(rec_rows)
+    rows["zone_rec_begin"] = np.concatenate([[0], np.cumsum([len(rs) for rs in keep])]).astype(np.uint32)
+    return dict(rows=compact_actual(rows),
+                lb_target=np.concatenate([lb_upd, np.full(len(lb_add), GAR_NONE)]).astype(np.uint32),
+                acc_target=np.concatenate([acc_upd, np.full(len(acc_add), GAR_NONE)]).astype(np.uint32),
+                zone_target=zones.astype(np.uint32), lb_deleted=lb_del.astype(np.uint32), acc_deleted=acc_del.astype(np.uint32))
+
+
+def actual_struct(cols: dict):
+    """(Snapshot owning the buffers, its GarActual) for an actual column dict: the `rows` of Engine.apply_actual."""
+    empty_objects = {c: np.zeros(0 if not isinstance(k, tuple) else 1, dtype=np.uint32 if isinstance(k, tuple) else tables._DT[k])
+                     for t, (_, cl) in tables.OBJ_TABLES.items() for c, k in cl}
+    empty_objects["slab"] = np.zeros(0, dtype=np.uint8)
+    snap = tables.from_columns(empty_objects, cols)
+    return snap, snap.actual
+
+
 def objects_struct(cols: dict):
     """(Snapshot owning the buffers, its GarObjects) for an object column dict: the `upserts` of Engine.apply_objects."""
     empty_actual = {c: np.zeros(0 if not isinstance(k, tuple) else 1, dtype=np.uint32 if isinstance(k, tuple) else tables._DT[k])

@@ -420,6 +420,51 @@ typedef struct gar_delta_result {  /* arrays are caller-allocated */
 } gar_delta_result;
 int gar_snapshot_apply_objects(gar_engine *e, const gar_object_delta *d, gar_delta_result *out);
 
+/* ---------------------------------------------------------------- AWS deltas: re-listed AWS resources
+   What a worker re-lists after executing ops (or after a requeue) applied to the loaded AWS tables on the device, so that the
+   next batch diffs against what it just did instead of a stale list, without a reload.  The units are the list calls:
+     load balancer   one DescribeLoadBalancers row                                        addressed by resident LB row
+     accelerator     DescribeAccelerator + ListTagsForResource + ListListeners + ListEndpointGroups: the whole subtree
+                     (tags, listeners, port ranges, endpoint groups, endpoints)          addressed by resident accelerator row
+     hosted zone     ListResourceRecordSets(zone): the zone's complete record list        addressed by resident zone row
+   (Adding or removing hosted zones is a reload.)  Rules:
+     - order preserving: list order is part of the contract (the first (region, name) LB row wins, an owner's accelerators
+       are visited in list order, the first matching alias in a zone wins).  Deleted LB and accelerator rows are removed and
+       the survivors keep their relative order; a replaced row keeps its position; appended rows follow in delta order.  The
+       new row of resident row r is r - #{deleted rows < r}; listeners, endpoint groups, records and values follow their
+       parents exactly as a gar_snapshot_load of the resulting tables would lay them out, so the caller can compute every new
+       row from its own data.  The result carries the table sizes as a cross-check;
+     - a resident row appears at most once across the *_target and *_deleted arrays of its table, every row is < the table's
+       size, zone_target entries are distinct, and delta zone k's zone_name equals resident zone zone_target[k]'s name byte
+       for byte; otherwise GAR_E_INVALID;
+     - the strings of `rows` are appended to the resident AWS slab at a 16-byte aligned slab_base (append-only, as for
+       objects; slab_len tells the caller when a reload is worth it).
+   Atomic: `rows` passes the checks gar_snapshot_load applies to an actual table (enums, monotone CSRs, strings inside its
+   slab), and the rules above hold, before anything resident changes; on GAR_E_INVALID the snapshot is unchanged.  GAR_E_STATE
+   in the same cases as gar_snapshot_apply_objects; after a CUDA error in the middle no snapshot is loaded.  Every later gar_diff,
+   gar_diff_device, gar_diff_keys and gar_bindings_diff answers bit for bit as after a gar_snapshot_load of the same object table
+   and the resulting AWS tables; object and AWS deltas may interleave freely.  The call drops the prepared state (digests,
+   indexes) and the recorded launch sequence: the next diff prepares the snapshot as the first diff after a load does. */
+typedef struct gar_actual_delta {
+  const gar_actual *rows;          /* new rows: a complete actual table with its own slab, packed like a load's; NULL = none.  Its
+                                      LBs and accelerators (with their subtrees) replace or append; its zone k carries the new
+                                      record list of resident zone zone_target[k] and must have that zone's name */
+  const uint32_t *lb_target;       /* [rows->n_lbs]    resident LB row replaced by delta row k, or GAR_NONE = append */
+  const uint32_t *acc_target;      /* [rows->n_accels] the same for accelerators (the whole subtree is replaced) */
+  const uint32_t *zone_target;     /* [rows->n_zones]  resident zone row whose record list is replaced */
+  uint32_t n_lb_deleted;
+  const uint32_t *lb_deleted;      /* [n_lb_deleted]  resident LB rows */
+  uint32_t n_acc_deleted;
+  const uint32_t *acc_deleted;     /* [n_acc_deleted] resident accelerator rows */
+} gar_actual_delta;
+typedef struct gar_actual_delta_result {
+  uint32_t n_lbs, n_accels, n_tags, n_listeners, n_port_ranges, n_egs, n_endpoints, n_records, n_values; /* after the delta */
+  uint64_t slab_base;              /* offset of this delta's slab inside the resident AWS slab (16-byte aligned); 0 when `rows`
+                                      is NULL or holds no LB, accelerator or zone */
+  uint64_t slab_len;               /* resident AWS slab bytes after the delta, strings of replaced rows included */
+} gar_actual_delta_result;
+int gar_snapshot_apply_actual(gar_engine *e, const gar_actual_delta *d, gar_actual_delta_result *out);
+
 /* ---------------------------------------------------------------- EndpointGroupBinding set-diff (SURVEY.md §8 row f3)
    The third controller's decisions (pkg/controller/endpointgroupbinding/reconcile.go:20-217): finalizer handling and the
    set difference between the load balancers of the referenced Service/Ingress and status.endpointIds.  Evaluated against
