@@ -3,7 +3,7 @@
 // Shared by the CUDA backend (gar_engine.cu) and the host simulation (tests/hostsim), like gar_shard.h: functors for the
 // data-parallel steps plus a driver template, Splicer<B>, that runs them over a Backend.  Data movement of one delta:
 //   1. the keys of the delta (deletes, then upserts) are resolved against the resident ix_obj index on the device, one
-//      thread per key with a full key compare after the tag (as object_in_cache does);
+//      thread per key with a full key compare after the tag (as find_object does);
 //   2. the host turns the resolved rows into the delete / swap-move / replace / append sequence of include/garecon.h:
 //      O(batch) work that yields a short list of (new row <- source) overrides on top of the identity map;
 //   3. the upsert table is copied to the device; its slab is appended to the resident object slab (16-byte aligned);

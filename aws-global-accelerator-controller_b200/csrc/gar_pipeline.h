@@ -47,7 +47,8 @@ enum Slot {
   S_IX_LB, S_IX_OWNER = S_IX_LB + 3, S_IX_THOST = S_IX_OWNER + 3, S_IX_ZONE = S_IX_THOST + 3, S_IX_VAL = S_IX_ZONE + 3,
   S_IX_ALIAS = S_IX_VAL + 3, S_IX_OBJ = S_IX_ALIAS + 3, S_IX_OVN = S_IX_OBJ + 3,
   S_SORT_KEYS = S_IX_OVN + 3, S_SORT_VALS, S_SORT_KEYS_ALT, S_SORT_VALS_ALT, S_SORT_TAGS,
-  S_COUNTS, S_STATUS_GA, S_STATUS_R53, S_OPS, S_ERRFLAG, S_IX_EG, S_IX_EG_ENT, S_IX_EG_PAD, S_ACC_CLAIMED,
+  S_COUNTS, S_STATUS_GA, S_STATUS_R53, S_OPS, S_ERRFLAG, S_IX_EG, S_IX_EG_ENT, S_IX_EG_PAD,
+  S_VAL_OBJ, S_ACC_OBJ, S_OBJ_CANON, S_OWN_BEGIN, S_OWN_FILL, S_OWN_ENT, S_OWN_MULTI,
   S_IXA_BEGIN, S_IXA_FILL, S_IXA_ENT, S_IXA_MULTI, S_OVN_FILL, S_OVN_MULTI, S_LB_HASH, S_REC_FLAGS,
   S_NSLOTS
 };
@@ -62,6 +63,7 @@ struct FClassify {
   u32 *errflag;
   GAR_HD void operator()(u32 i) const {
     classify_object(T, W, i);
+    W.obj_canon[i] = i;  // rows that repeat an earlier row's key are redirected when ix_obj is ordered (canon_bucket)
     u32 dv = W.derived[i];
     if (dv & OBJ_KEY_BAD) GAR_ATOMIC_ADD(errflag, 1u);
     derived_public[i] = dv & 0xFFu;
@@ -362,6 +364,16 @@ struct FRowOvn {
 // IDX_SMALL_BUCKET (a hot key / adversarial input) raise `overflow`; the pipeline then rebuilds with the stable
 // radix sort (idx_gather).
 constexpr u32 IDX_SMALL_BUCKET = 48;
+// ix_obj only: the ordering pass also writes the duplicate-key exceptions of Work::obj_canon (buckets [b0, b1) of the begin
+// array it orders are ix_obj buckets; canon == nullptr: none)
+struct CanonHook {
+  u32 *canon;
+  const u8 *slab;
+  u32 b0, b1;
+  GAR_HD void operator()(u32 b, const IdxEntry *ent, u32 lo, u32 m) const {
+    if (canon && b >= b0 && b < b1) canon_bucket(ent, lo, m, slab, canon);
+  }
+};
 template <class RowF>
 struct FIdxRows {
   RowF rowf;
@@ -405,6 +417,7 @@ struct FIdxOrder {
   const u32 *begin;
   IdxEntry *ent;
   u32 *overflow;
+  CanonHook canon;
   GAR_HD void operator()(u32 b) const {
     u32 lo = begin[b], m = begin[b + 1] - lo;
     if (m < 2) return;
@@ -421,6 +434,7 @@ struct FIdxOrder {
       }
       if (j != k) ent[lo + j] = x;
     }
+    canon(b, ent, lo, m);
   }
 };
 struct FIdxGather {  // radix fallback: position p of the stable sorted order holds row vals[p]
@@ -430,6 +444,15 @@ struct FIdxGather {  // radix fallback: position p of the stable sorted order ho
   IdxEntry *ent;
   GAR_HD void operator()(u32 p) const {
     if (p < *nvalid) ent[p] = tmp[vals[p]];
+  }
+};
+struct FIdxCanon {  // radix fallback of ix_obj: the duplicate-key pass over the (already ordered) buckets
+  const u32 *begin;
+  const IdxEntry *ent;
+  CanonHook canon;
+  GAR_HD void operator()(u32 b) const {
+    const u32 lo = begin[b], m = begin[b + 1] - lo;
+    if (m >= 2) canon(b, ent, lo, m);
   }
 };
 // One-pass build (the default): the row-local passes have already counted every bucket (Work::hist); after ONE scan over the
@@ -480,10 +503,11 @@ struct FIdxMultiList {
   }
 };
 struct FIdxOrderMulti {
-  const u32 *begin;  // the group's whole bucket array
+  const u32 *begin;  // the group's whole bucket array (or the owned lists' segment array)
   IdxEntry *ent;
   const u32 *multi;
   u32 *overflow;
+  CanonHook canon;
   GAR_HD void operator()(u32 t) const {
     const u32 b = multi[1 + t];
     const u32 lo = begin[b], m = begin[b + 1] - lo;
@@ -500,6 +524,7 @@ struct FIdxOrderMulti {
       }
       if (j != k) ent[lo + j] = x;
     }
+    canon(b, ent, lo, m);
   }
 };
 // everything the host reads back at the END of a diff, gathered into one small block (no read-back in the middle)
@@ -529,20 +554,89 @@ struct FGatherHeader {
   GAR_HD void operator()(u32) const { flags[FW_NDPORTS] = *ndports; }
 };
 // the two per-value joins in one pass (independent probe chains overlap): first alias record under the value's (zone, name),
-// and whether the owner the value names is still in the object cache
+// and the object the value names (which also says whether it is an orphan)
 struct FValueJoins {
   DevTables T;
   Work W;
   GAR_HD void operator()(u32 v) const {
     link_value_alias(T, W, v);
-    mark_orphan_value(T, W, v);
+    resolve_value(T, W, v);
   }
 };
 // the object half of FValueJoins, alone: re-run after an object delta (the alias links read the actual side only)
-struct FMarkOrphanValue {
+struct FResolveValue {
   DevTables T;
   Work W;
-  GAR_HD void operator()(u32 v) const { mark_orphan_value(T, W, v); }
+  GAR_HD void operator()(u32 v) const { resolve_value(T, W, v); }
+};
+struct FResolveAccel {
+  DevTables T;
+  Work W;
+  GAR_HD void operator()(u32 a) const { resolve_accel(T, W, a); }
+};
+// owned-list records (payloads: gar_rows.h "index probes"): x < nacc is accelerator x, else owner value x - nacc
+GAR_HD IdxEntry own_entry(const DevTables &T, const Work &W, u32 x) {
+  IdxEntry e;
+  e.tag = e.a0 = e.a1 = 0;
+  e.s0 = e.s1 = 0;
+  if (x < T.a.n_accels) {
+    e.row = x;
+    return e;
+  }
+  const u32 v = x - T.a.n_accels, rec = W.val_rec[v];
+  const ValLink l = W.val_link[v];
+  e.tag = l.alias_row;
+  e.row = v;
+  e.a0 = rec;
+  e.a1 = W.rec_zone[rec] | ((W.rec_flags[rec] & 1) ? VALNAME_HAS_BACKSLASH : 0u);
+  e.s0 = l.alias_dns;
+  e.s1 = T.a.rec_name[rec];
+  return e;
+}
+// segment of row x (accelerators first, then values) in the owned lists; 2n: not on any list
+GAR_HD u32 own_segment(const DevTables &T, const Work &W, u32 x) {
+  const u32 nacc = T.a.n_accels;
+  const u32 o = x < nacc ? W.acc_obj[x] : W.val_obj[x - nacc];
+  return o == GAR_NONE ? 2 * T.o.n_objects : 2 * o + (x < nacc ? 0u : 1u);
+}
+// placement into the scanned segments through per-segment cursors (one atomic), rows of a segment in any order: FIdxOrderMulti
+// orders the segments with two or more rows afterwards
+struct FOwnPlace {
+  DevTables T;
+  Work W;
+  u32 *cursor;
+  IdxEntry *ent;
+  u32 x0;  // 0: accelerators, n_accels: values
+  GAR_HD void operator()(u32 i) const {
+    const u32 x = x0 + i, k = own_segment(T, W, x);
+    if (k == 2 * T.o.n_objects) return;
+#if defined(__CUDA_ARCH__)
+    const u32 pos = atomicAdd(&cursor[k], 1u);
+#else
+    const u32 pos = cursor[k]++;
+#endif
+    ent[pos] = own_entry(T, W, x);
+  }
+};
+// radix fallback (some list is longer than IDX_SMALL_BUCKET): (segment, x) pairs, stably sorted, then gathered
+struct FOwnKeys {
+  DevTables T;
+  Work W;
+  u32 *keys, *vals;
+  GAR_HD void operator()(u32 x) const {
+    keys[x] = own_segment(T, W, x);
+    vals[x] = x;
+  }
+};
+struct FOwnGather {
+  DevTables T;
+  Work W;
+  const u32 *vals;
+  const u32 *total;
+  IdxEntry *ent;
+  GAR_HD void operator()(u32 p) const {
+    if (p < *total) ent[p] = own_entry(T, W, vals[p]);
+  }
 };
 
 // --- count / emit.  counts layout: [GA obj: n][GA orphan: nacc][R53 obj: n][orphan alias: nrec][orphan value: nval][total]
@@ -814,7 +908,7 @@ struct Pipeline {
 
   // nb: buckets (power of two).  load: target rows per bucket used to size nb from the row count.
   template <class RowF>
-  HashIdx build_index(int slot, u32 nrows, u32 load, RowF rowf, u32 *overflow, bool force_radix) {
+  HashIdx build_index(int slot, u32 nrows, u32 load, RowF rowf, u32 *overflow, bool force_radix, CanonHook canon = {}) {
     u32 nb = next_pow2(nrows / load < 16 ? 16 : nrows / load);
     u32 *keys = (u32 *)be.ensure(S_SORT_KEYS, sizeof(u32) * (size_t)(nrows + 1));
     u32 *vals = (u32 *)be.ensure(S_SORT_VALS, sizeof(u32) * (size_t)(nrows + 1));
@@ -828,12 +922,13 @@ struct Pipeline {
       u32 *cursor = (u32 *)be.ensure(S_SORT_KEYS_ALT, sizeof(u32) * (size_t)(nb + 1));
       be.copy32(cursor, begin, nb);
       be.for_each("idx_place", nrows, FIdxPlace{keys, cursor, tmp, ent, nb});
-      be.for_each("idx_order", nb, FIdxOrder{begin, ent, overflow});
+      be.for_each("idx_order", nb, FIdxOrder{begin, ent, overflow, canon});
     } else if (nrows) {
       u32 *keys2 = (u32 *)be.ensure(S_SORT_KEYS_ALT, sizeof(u32) * (size_t)(nrows + 1));
       u32 *vals2 = (u32 *)be.ensure(S_SORT_VALS_ALT, sizeof(u32) * (size_t)(nrows + 1));
       be.sort_pairs(keys, vals, keys2, vals2, nrows, ilog2(nb) + 1);
       be.for_each("idx_gather", nrows, FIdxGather{vals, begin + nb, tmp, ent});
+      if (canon.canon) be.for_each("idx_order", nb, FIdxCanon{begin, ent, canon});
     }
     return HashIdx{begin, ent, nb - 1};
   }
@@ -865,7 +960,9 @@ struct Pipeline {
     W.r53_mode = (u8 *)be.ensure(S_R53_MODE, (size_t)n + 1);
     W.r53_acc = (u32 *)be.ensure(S_R53_ACC, 4 * (size_t)(n + 1));
     W.r53_acc_dns = (gar_str *)be.ensure(S_R53_ACC_DNS, 8 * (size_t)(n + 1));
+    W.obj_canon = (u32 *)be.ensure(S_OBJ_CANON, 4 * (size_t)(n + 1));
   }
+  CanonHook canon_hook(u32 b0, u32 b1) const { return CanonHook{W.obj_canon, T.o.slab, b0, b1}; }
   void alloc_work() {
     const u32 nacc = T.a.n_accels, nrec = T.a.n_records, nval = T.a.n_values;
     alloc_obj_work();
@@ -883,6 +980,8 @@ struct Pipeline {
     W.val_cls = (u8 *)be.ensure(S_VAL_CLS, nval + 1);
     W.val_key = (gar_str *)be.ensure(S_VAL_KEY, 8 * (size_t)(nval + 1));
     W.val_orphan = (u8 *)be.ensure(S_VAL_ORPHAN, nval + 1);
+    W.val_obj = (u32 *)be.ensure(S_VAL_OBJ, 4 * (size_t)(nval + 1));
+    W.acc_obj = (u32 *)be.ensure(S_ACC_OBJ, 4 * (size_t)(nacc + 1));
     W.val_link = (ValLink *)be.ensure(S_VAL_LINK, sizeof(ValLink) * (size_t)(nval + 1));
     W.acc_digest = (AccDigest *)be.ensure(S_ACC_DIGEST, sizeof(AccDigest) * (size_t)(nacc + 1));
     W.lb_hash = (u64 *)be.ensure(S_LB_HASH, 8 * (size_t)(T.a.n_lbs + 1));
@@ -894,7 +993,6 @@ struct Pipeline {
     be.fill32(errflag, 0, FW_WORDS);
     W.acc_guest_from = acc_guest_from;
     W.sharded = sharded;
-    W.acc_claimed = nullptr;
   }
   void stage1() {
     const u32 n = T.o.n_objects, nlbi = T.o.n_lbi, nacc = T.a.n_accels, nrec = T.a.n_records, nval = T.a.n_values;
@@ -966,37 +1064,82 @@ struct Pipeline {
     be.fill32(ixa_multi, 0, 1);
     const IxPlan &P = planA;
     auto n = [&](int k) { return P.want[k] ? P.rows[k] : 0u; };
-    be.for_each_multi("idx_place", {n(IX_LB), n(IX_OWNER), n(IX_THOST), n(IX_ZONE), n(IX_VAL), n(IX_ALIAS), n(IX_OBJ), P.total_nb},
-                      placer(IX_LB, FRowLb{T, W}), placer(IX_OWNER, FRowOwner{T, W}), placer(IX_THOST, FRowThost{T, W}), placer(IX_ZONE, FRowZone{T}),
-                      placer(IX_VAL, FRowVal{T, W}), placer(IX_ALIAS, FRowAlias{T, W}), placer(IX_OBJ, FRowObj{T, W}), FIdxMultiList{ixa_begin, ixa_multi});
-    be.for_each_dyn("idx_order", ixa_multi, multi_cap, FIdxOrderMulti{ixa_begin, ixa_ent, ixa_multi, overflow});
+    be.for_each_multi("idx_place", {n(IX_LB), n(IX_THOST), n(IX_ZONE), n(IX_ALIAS), n(IX_OBJ), P.total_nb},
+                      placer(IX_LB, FRowLb{T, W}), placer(IX_THOST, FRowThost{T, W}), placer(IX_ZONE, FRowZone{T}),
+                      placer(IX_ALIAS, FRowAlias{T, W}), placer(IX_OBJ, FRowObj{T, W}), FIdxMultiList{ixa_begin, ixa_multi});
+    const CanonHook canon = P.want[IX_OBJ] ? canon_hook(P.off[IX_OBJ], P.off[IX_OBJ] + P.nb[IX_OBJ]) : CanonHook{};
+    be.for_each_dyn("idx_order", ixa_multi, multi_cap, FIdxOrderMulti{ixa_begin, ixa_ent, ixa_multi, overflow, canon});
     if (P.want[IX_LB]) W.ix_lb = group_a_index(IX_LB);
-    if (P.want[IX_OWNER]) W.ix_owner = group_a_index(IX_OWNER);
     if (P.want[IX_THOST]) W.ix_thost = group_a_index(IX_THOST);
     if (P.want[IX_ZONE]) W.ix_zone = group_a_index(IX_ZONE);
-    if (P.want[IX_VAL]) W.ix_val = group_a_index(IX_VAL);
     if (P.want[IX_ALIAS]) W.ix_alias = group_a_index(IX_ALIAS);
     if (P.want[IX_OBJ]) W.ix_obj = group_a_index(IX_OBJ);
   }
-  // the orphan-value index: its keys exist only after the per-value joins (which count its buckets: mark_orphan_value)
-  void arm_ovn() {
-    ovn_nb = next_pow2(T.a.n_values / 8 < 16 ? 16 : T.a.n_values / 8);
-    u32 *cnt = (u32 *)be.ensure(S_IX_OVN + 0, 4 * (size_t)(ovn_nb + 2));
-    be.fill32(cnt, 0, (size_t)ovn_nb + 2);
-    W.hist[IX_OVN] = IxHist{cnt, ovn_nb - 1};
+  // ---- the owner-keyed joins, resolved from the AWS side (after ix_obj and its obj_canon exist): one fused pass over values
+  // (alias links when `link_aliases`, object row, orphan mark) and owner-keyed accelerators (object row) counts the owned-list
+  // segments and the buckets of the orphan-value index, whose keys exist only now; then both are built the way group A is:
+  // one scan each, one fused placement through cursors, ordering of the segments / buckets with two or more rows.
+  void resolve_owners(bool link_aliases) {
+    const u32 n = T.o.n_objects, nacc = T.a.n_accels, nval = T.a.n_values, nseg = 2 * n;
+    u32 *overflow = errflag + FW_IDX_OVERFLOW;
+    W.own_begin = (u32 *)be.ensure(S_OWN_BEGIN, 4 * (size_t)(nseg + 2));
+    be.fill32(W.own_begin, 0, (size_t)nseg + 1);
+    u32 *ovn = nullptr;
+    if (!force_radix) {
+      ovn_nb = next_pow2(nval / 8 < 16 ? 16 : nval / 8);
+      ovn = (u32 *)be.ensure(S_IX_OVN + 0, 4 * (size_t)(ovn_nb + 2));
+      be.fill32(ovn, 0, (size_t)ovn_nb + 2);
+      W.hist[IX_OVN] = IxHist{ovn, ovn_nb - 1};
+    } else {
+      W.hist[IX_OVN] = IxHist{nullptr, 0};
+    }
+    if (link_aliases) be.for_each_multi("value_joins", {nval, nacc}, FValueJoins{T, W}, FResolveAccel{T, W});
+    else be.for_each_multi("resolve_owners", {nval, nacc}, FResolveValue{T, W}, FResolveAccel{T, W});
+    be.exclusive_scan(W.own_begin, nseg + 1);  // [nseg] = number of records
+    IdxEntry *own = (IdxEntry *)be.ensure(S_OWN_ENT, sizeof(IdxEntry) * ((size_t)nacc + nval + 1));
+    if (!force_radix) {
+      be.exclusive_scan(ovn, ovn_nb + 1);
+      u32 *ovn_cursor = (u32 *)be.ensure(S_OVN_FILL, 4 * (size_t)(ovn_nb + 1));
+      IdxEntry *ovn_ent = (IdxEntry *)be.ensure(S_IX_OVN + 1, sizeof(IdxEntry) * (size_t)(nval + 1));
+      u32 *ovn_multi = (u32 *)be.ensure(S_OVN_MULTI, 4 * (size_t)(nval / 2 + 3));
+      u32 *own_cursor = (u32 *)be.ensure(S_OWN_FILL, 4 * (size_t)(nseg + 1));
+      const u32 own_multi_cap = (u32)(((u64)nacc + nval) / 2 + 1);
+      u32 *own_multi = (u32 *)be.ensure(S_OWN_MULTI, 4 * (size_t)(own_multi_cap + 2));
+      be.copy32(ovn_cursor, ovn, (size_t)ovn_nb + 1);
+      be.copy32(own_cursor, W.own_begin, (size_t)nseg + 1);
+      be.fill32(ovn_multi, 0, 1);
+      be.fill32(own_multi, 0, 1);
+      be.for_each_multi("idx_place", {nval, ovn_nb, nacc, nval, nseg}, FIdxPlaceDirect<FRowOvn>{FRowOvn{T, W}, ovn_cursor, ovn_ent, ovn_nb - 1},
+                        FIdxMultiList{ovn, ovn_multi}, FOwnPlace{T, W, own_cursor, own, 0}, FOwnPlace{T, W, own_cursor, own, nacc},
+                        FIdxMultiList{W.own_begin, own_multi});
+      be.for_each_dyn("idx_order", ovn_multi, nval / 2 + 1, FIdxOrderMulti{ovn, ovn_ent, ovn_multi, overflow});
+      be.for_each_dyn("idx_order", own_multi, own_multi_cap, FIdxOrderMulti{W.own_begin, own, own_multi, overflow});
+      W.ix_ovn = HashIdx{ovn, ovn_ent, ovn_nb - 1};
+    } else {  // a list longer than IDX_SMALL_BUCKET: (segment, row) pairs through the stable radix sort
+      const u32 nx = nacc + nval;
+      u32 *keys = (u32 *)be.ensure(S_SORT_KEYS, 4 * (size_t)(nx + 1));
+      u32 *vals = (u32 *)be.ensure(S_SORT_VALS, 4 * (size_t)(nx + 1));
+      u32 *keys2 = (u32 *)be.ensure(S_SORT_KEYS_ALT, 4 * (size_t)(nx + 1));
+      u32 *vals2 = (u32 *)be.ensure(S_SORT_VALS_ALT, 4 * (size_t)(nx + 1));
+      if (nx) {
+        be.for_each("own_keys", nx, FOwnKeys{T, W, keys, vals});
+        be.sort_pairs(keys, vals, keys2, vals2, nx, ilog2(nseg + 1) + 1);
+        be.for_each("own_gather", nx, FOwnGather{T, W, vals, W.own_begin + nseg, own});
+      }
+      W.ix_ovn = build_index(S_IX_OVN, nval, 8, FRowOvn{T, W}, overflow, true);
+    }
+    W.own = own;
+    owners_stale = false;
   }
-  void finish_ovn() {
-    const u32 nval = T.a.n_values;
-    u32 *begin = W.hist[IX_OVN].cnt;
-    be.exclusive_scan(begin, ovn_nb + 1);
-    u32 *cursor = (u32 *)be.ensure(S_OVN_FILL, 4 * (size_t)(ovn_nb + 1));
-    IdxEntry *ent = (IdxEntry *)be.ensure(S_IX_OVN + 1, sizeof(IdxEntry) * (size_t)(nval + 1));
-    u32 *multi = (u32 *)be.ensure(S_OVN_MULTI, 4 * (size_t)(nval / 2 + 3));
-    be.copy32(cursor, begin, (size_t)ovn_nb + 1);
-    be.fill32(multi, 0, 1);
-    be.for_each_multi("idx_place", {nval, ovn_nb}, FIdxPlaceDirect<FRowOvn>{FRowOvn{T, W}, cursor, ent, ovn_nb - 1}, FIdxMultiList{begin, multi});
-    be.for_each_dyn("idx_order", multi, nval / 2 + 1, FIdxOrderMulti{begin, ent, multi, errflag + FW_IDX_OVERFLOW});
-    W.ix_ovn = HashIdx{begin, ent, ovn_nb - 1};
+  // ix_owner / ix_val: what a key that LEFT the cache owns (gar_diff_keys' deleted keys; objects in the cache read their owned
+  // lists).  Built the first time a diff carries deleted keys; they read the AWS side only, so they stay until it changes.
+  bool owner_indexes = false;
+  void build_owner_indexes() {
+    if (owner_indexes) return;
+    u32 *overflow = errflag + FW_IDX_OVERFLOW;
+    W.ix_owner = build_index(S_IX_OWNER, T.a.n_accels, 1, FRowOwner{T, W}, overflow, force_radix);
+    W.ix_val = build_index(S_IX_VAL, T.a.n_values, 1, FRowVal{T, W}, overflow, force_radix);
+    owner_indexes = true;
   }
 
   // what the sharded mode's routing needs of a rank's slice: the row-local pass + the (zone, name) -> alias record index
@@ -1020,33 +1163,26 @@ struct Pipeline {
   u64 ops_cap = 0;
   bool tiny_caps = false;  // test hook (environment GAR_TINY_CAPS=1): start every capacity at 1 so that the grow-and-rerun paths run
   int prepare() {
-    const u32 n = T.o.n_objects, nacc = T.a.n_accels, nzone = T.a.n_zones, nrec = T.a.n_records, nval = T.a.n_values;
+    const u32 n = T.o.n_objects, nacc = T.a.n_accels, nzone = T.a.n_zones, nrec = T.a.n_records;
     alloc_work();
-    if (!force_radix) {
-      arm_group_a((1u << IX_OVN) - 1);
-      arm_ovn();
-    }
+    if (!force_radix) arm_group_a((1u << IX_LB) | (1u << IX_THOST) | (1u << IX_ZONE) | (1u << IX_ALIAS) | (1u << IX_OBJ));
     stage1();
     listen_ports();
 
-    // stage 3: hash indexes
+    // stage 3: hash indexes, then the owner-keyed joins
     u32 *overflow = errflag + FW_IDX_OVERFLOW;
     if (!force_radix) {
       finish_group_a();
-      if (nval) be.for_each("value_joins", nval, FValueJoins{T, W});
-      finish_ovn();
-    } else {  // some bucket was too large for the per-bucket ordering: every index through the stable radix sort
+    } else {  // some bucket or owned list was too large for the per-bucket ordering: everything through the stable radix sort
       W.ix_lb = build_index(S_IX_LB, T.a.n_lbs, 1, FRowLb{T, W}, overflow, true);
-      W.ix_owner = build_index(S_IX_OWNER, nacc, 1, FRowOwner{T, W}, overflow, true);
       W.ix_thost = build_index(S_IX_THOST, nacc, 1, FRowThost{T, W}, overflow, true);
       W.ix_zone = build_index(S_IX_ZONE, nzone, 1, FRowZone{T}, overflow, true);
-      W.ix_val = build_index(S_IX_VAL, nval, 1, FRowVal{T, W}, overflow, true);
       W.ix_alias = build_index(S_IX_ALIAS, nrec, 2, FRowAlias{T, W}, overflow, true);
-      W.ix_obj = build_index(S_IX_OBJ, n, 1, FRowObj{T, W}, overflow, true);
-      if (nval) be.for_each("value_joins", nval, FValueJoins{T, W});
-      W.ix_ovn = build_index(S_IX_OVN, nval, 8, FRowOvn{T, W}, overflow, true);
+      W.ix_obj = build_index(S_IX_OBJ, n, 1, FRowObj{T, W}, overflow, true, canon_hook(0, 0xFFFFFFFFu));
     }
-    obj_stale = ovn_stale = false;
+    resolve_owners(true);
+    obj_stale = false;
+    owner_indexes = false;
     return GAR_OK;
   }
   // stage 2: listen-ports annotation -> desired port lists (count, scan, write).  The total stays on the device: the list
@@ -1064,12 +1200,14 @@ struct Pipeline {
   }
 
   // ---- object deltas (gar_delta.h).  The prepared state splits in two halves:
-  //   actual side  digests, LB hashes, zone mask, records / values, the LB / owner / target-hostname / zone / value / alias
-  //                indexes and the value -> alias links: depend on the AWS tables only and stay resident across deltas;
-  //   object side  classify, tokenise, listen ports, ix_obj, and (for the full diff's orphan sweep only) the orphan value
-  //                marks + ix_ovn: rebuilt over the whole resident table after a delta.
-  // obj_stale: the object table changed since the object side was built.  ovn_stale: the orphan values lag behind ix_obj.
-  bool obj_stale = false, ovn_stale = false;
+  //   actual side  digests, LB hashes, zone mask, records / values, the LB / target-hostname / zone / alias indexes, the
+  //                value -> alias links and the on-demand ix_owner / ix_val: depend on the AWS tables only and stay resident
+  //                across deltas;
+  //   object side  classify, tokenise, listen ports, ix_obj + obj_canon, and the owner-keyed joins that point into the object
+  //                rows (val_obj / acc_obj, the owned lists, the orphan value marks + ix_ovn): rebuilt over the whole resident
+  //                table after a delta.
+  // obj_stale: the object table changed since the object side was built.  owners_stale: the owner-keyed joins lag behind ix_obj.
+  bool obj_stale = false, owners_stale = false;
   void prepare_objects() {
     const u32 n = T.o.n_objects, nlbi = T.o.n_lbi;
     alloc_obj_work();
@@ -1079,22 +1217,9 @@ struct Pipeline {
     if (n) be.for_each("classify_objects", n, FClassify{T, W, derived_public, nullptr, errflag});
     if (nlbi) be.for_each_staged("tokenise_hostnames", nlbi, FTokenise{T, W});
     listen_ports();
-    W.ix_obj = build_index(S_IX_OBJ, n, 1, FRowObj{T, W}, errflag + FW_IDX_OVERFLOW, force_radix);
+    W.ix_obj = build_index(S_IX_OBJ, n, 1, FRowObj{T, W}, errflag + FW_IDX_OVERFLOW, force_radix, canon_hook(0, 0xFFFFFFFFu));
     obj_stale = false;
-    ovn_stale = true;
-  }
-  void prepare_orphan_values() {
-    const u32 nval = T.a.n_values;
-    if (!force_radix) {
-      arm_ovn();
-      if (nval) be.for_each("orphan_values", nval, FMarkOrphanValue{T, W});
-      finish_ovn();
-    } else {
-      W.hist[IX_OVN] = IxHist{nullptr, 0};
-      if (nval) be.for_each("orphan_values", nval, FMarkOrphanValue{T, W});
-      W.ix_ovn = build_index(S_IX_OVN, nval, 8, FRowOvn{T, W}, errflag + FW_IDX_OVERFLOW, true);
-    }
-    ovn_stale = false;
+    owners_stale = true;
   }
   // a complete ix_obj of the current object table (key resolution of a delta), with the same index-overflow fallback as run_with
   int index_objects() {
@@ -1149,8 +1274,6 @@ struct Pipeline {
     gar_op *stage_r53 = (gar_op *)be.ensure(S_STAGE_R53, sizeof(gar_op) * ((size_t)n * OPS_STAGE_CAP + 1));
     u32 *st_ga = (u32 *)be.out_status_ga(n);
     u32 *st_r53 = (u32 *)be.out_status_r53(n);
-    W.acc_claimed = (u8 *)be.ensure(S_ACC_CLAIMED, (size_t)nacc + 4);
-    be.fill32((u32 *)W.acc_claimed, 0, ((size_t)nacc + 3) / 4);
     if (n) be.for_each_warp("ga_objects", n, FGaObj{T, W, counts + L.ga_obj(0), stage_ga, st_ga, nullptr});
     r53_relational(n, nullptr, st_r53);
     if (n) be.for_each_warp("r53_objects", n, FR53Obj{T, W, counts + L.r53_obj(0), stage_r53, st_r53, nullptr});
@@ -1171,7 +1294,6 @@ struct Pipeline {
     if (orphan_sweep)
       be.for_each_multi("orphans_emit", {nacc, nrec, nval}, FGaOrphan{T, W, L, counts, ops, cap}, FR53OrphanAlias{T, W, L, counts, ops, cap},
                         FR53OrphanValue{T, W, L, counts, ops, cap});
-    W.acc_claimed = nullptr;  // other decide flavours (incremental, bindings) do not maintain it
     return GAR_OK;
   }
 
@@ -1188,6 +1310,7 @@ struct Pipeline {
     u32 *st_ga = (u32 *)be.out_status_ga(m);
     u32 *st_r53 = (u32 *)be.out_status_r53(m);
     u32 *derived_out = (u32 *)be.out_derived_keys(m);
+    if (nd) build_owner_indexes();
     if (m) {
       be.for_each("gather_derived", m, FGatherDerived{W.derived, rows, derived_out});
       be.for_each_warp("ga_objects", m, FGaObj{T, W, c_ga, stage_ga, st_ga, rows});
@@ -1240,7 +1363,7 @@ struct Pipeline {
     for (int attempt = 0; attempt < 8; attempt++) {
       u64 sig = 0;
       if (full) {
-        sig = hmix(hmix(prepared ? (obj_stale || ovn_stale ? 9 : 1) : 2, force_radix ? 3 : 4), hmix(hmix(dport_cap, pair_cap), ops_cap));
+        sig = hmix(hmix(prepared ? (obj_stale || owners_stale ? 9 : 1) : 2, force_radix ? 3 : 4), hmix(hmix(dport_cap, pair_cap), ops_cap));
         sig = hmix(sig, hmix(orphan_sweep ? 5 : 6, tiny_caps ? 7 : 8)) | 1;
       }
       const int g = full ? be.graph_begin(sig) : 0;
@@ -1248,7 +1371,7 @@ struct Pipeline {
       if (g != 2) {
         if (!prepared) rc = prepare();
         else if (obj_stale) prepare_objects();
-        if (rc == GAR_OK && full && ovn_stale) prepare_orphan_values();  // only the full diff's orphan sweep reads them
+        if (rc == GAR_OK && owners_stale) resolve_owners(false);  // the decide functions of every flavour read the owned lists
         if (rc == GAR_OK) rc = decide();
       }
       prepared = true;

@@ -99,7 +99,7 @@ struct Work {
   u32 dport_cap;   // capacity of dports
   // objects
   u32 *derived;        // [n] GAR_DV_* | OBJ_*
-  u64 *okey_hash;      // [n] key_hash_kinded(kind, "ns/name"): probes ix_owner / ix_val, builds ix_obj
+  u64 *okey_hash;      // [n] key_hash_kinded(kind, "ns/name"): builds ix_obj
   gar_str *ann_r53;    // [n] value of the route53-hostname annotation
   gar_str *ann_name;   // [n] value of global-accelerator-name
   gar_str *ann_tags;   // [n] value of global-accelerator-tags
@@ -132,7 +132,14 @@ struct Work {
   // and every row serves both.
   u32 acc_guest_from;
   u32 sharded;
-  u8 *acc_claimed;  // [n_accels] written by ga_reconcile (full diff only; nullptr otherwise), read by ga_orphan
+  // owner-keyed joins, resolved ONCE from the AWS side (the value pass): every owner value and every accelerator that
+  // acc_in_owner_index admits is resolved to its object's canonical row, and each canonical object gets the rows that name it
+  u32 *val_obj;    // [n_values] canonical object row of an owner value's (kind, key); GAR_NONE: no such object
+  u32 *acc_obj;    // [n_accels] the same for owner-keyed accelerators; GAR_NONE for the others
+  u32 *obj_canon;  // [n] the lowest row with the object's (kind, key) (rows of a load may repeat a key): whose lists it reads
+  u32 *own_begin;  // [2n+1] owned lists, two segments per canonical object o: accelerators [own_begin[2o], own_begin[2o+1]),
+                   // owner values [own_begin[2o+1], own_begin[2o+2]); each ascending by row (= list order)
+  const IdxEntry *own;  // owned-list records (payloads: "index probes" below)
   // route53 ensure, relational form (objects with exactly one lbIngress)
   u8 *r53_mode;        // [n] R53_MODE_*
   u32 *r53_acc;        // [n] the accelerator found by target hostname
@@ -145,12 +152,12 @@ struct Work {
   u32 *pair_rec;       // [n_pairs]
   // indexes
   HashIdx ix_lb;     // (region, name) -> LB rows
-  HashIdx ix_owner;  // (kind, "ns/name") -> accelerators that are ACC_MINE and ACC_OWNER_KEYED
+  HashIdx ix_owner;  // (kind, "ns/name") -> accelerators that are ACC_MINE and ACC_OWNER_KEYED  (deleted keys only, built on demand)
   HashIdx ix_thost;  // target hostname -> accelerators that are ACC_MINE
   HashIdx ix_zone;   // zone name without the trailing dot -> zone rows
   const u64 *zone_len_mask;  // [4] bit L set: some indexed zone name has L bytes (L >= 255 -> bit 255)
-  HashIdx ix_val;    // (kind, "ns/name") -> owner value rows of this cluster
-  HashIdx ix_alias;  // (zone, record name) -> alias record rows
+  HashIdx ix_val;    // (kind, "ns/name") -> owner value rows of this cluster  (deleted keys only, built on demand)
+  HashIdx ix_alias; // (zone, record name) -> alias record rows
   HashIdx ix_obj;    // (kind, "ns/name") -> object rows
   HashIdx ix_ovn;    // (zone, record name) -> orphan owner value rows
 };
@@ -493,6 +500,9 @@ GAR_HD void classify_value(const DevTables &T, const Work &W, u32 v) { classify_
 //   ix_alias  row=record a0=zone   a1=rec_type      s0=record name ref s1=alias dns ref
 //   ix_obj    row=object a0=kind                    s0="ns/name" ref
 //   ix_ovn    row=value a0=record  a1=zone          s0=record name ref s1=value ref
+// Owned-list records (Work::own; not a hash index, the same 32-byte entries so that the build reuses the index machinery):
+//   accelerator segment  row=accel
+//   value segment        row=value a0=record  a1=zone|backslash  tag=first alias A record row  s0=its alias DNS ref  s1=record name ref
 
 // GetLoadBalancer (load_balancer.go:13-30) on a client bound to `region` (aws.go:23-25): first row wins
 GAR_HD u32 find_lb(const DevTables &T, const Work &W, Str region, Str name, u32 *state) {
@@ -506,7 +516,21 @@ GAR_HD u32 find_lb(const DevTables &T, const Work &W, Str region, Str name, u32 
   return GAR_NONE;
 }
 
-// ListGlobalAcceleratorByResource (global_accelerator.go:87-110) as a cursor over ix_owner
+// ListGlobalAcceleratorByResource (global_accelerator.go:87-110) of an object in the cache: its canonical row's accelerator
+// segment, in ListAccelerators order (the value pass resolved kind and key, nothing is compared here)
+struct OwnRange {
+  u32 pos, end;
+};
+GAR_HD OwnRange own_accs(const Work &W, u32 i) {
+  const u32 s = 2 * W.obj_canon[i];
+  return OwnRange{W.own_begin[s], W.own_begin[s + 1]};
+}
+GAR_HD OwnRange own_vals(const Work &W, u32 i) {
+  const u32 s = 2 * W.obj_canon[i] + 1;
+  return OwnRange{W.own_begin[s], W.own_begin[s + 1]};
+}
+
+// ... and of a key that left the cache (deleted keys of gar_diff_keys), as a cursor over ix_owner
 struct OwnerIter {
   Cursor c;
   Str key;
@@ -620,21 +644,6 @@ GAR_HD u32 u_find_lb(const DevTables &T, const Work &W, bool active, Str region,
       *state = e.a0;
     }
   }
-  return found;
-}
-
-// next accelerator of the owner key (ListGlobalAcceleratorByResource, global_accelerator.go:87-110); the cursor
-// lives in the caller: one call = one accelerator, all lanes together
-GAR_HD u32 u_owner_next(const DevTables &T, const Work &W, bool active, u32 kind, Str key, Cursor &c) {
-  u32 found = GAR_NONE;
-  U_BUCKET_LOOP(active && found == GAR_NONE, c) {
-    IdxEntry e;
-    bool hit = u_bucket_step(W.ix_owner, active && found == GAR_NONE, c, &e);
-    hit = hit && (((e.a0 & ACC_OWNER_INGRESS) != 0) ? 1u : 0u) == kind;
-    if (u_streq(hit, mkstr(T.a.slab, e.s0), key)) found = e.row;
-  }
-  // an accelerator reached through its owner's object cannot be an orphan: the orphan pass skips its cache probe
-  if (found != GAR_NONE && W.acc_claimed) W.acc_claimed[found] = 1;
   return found;
 }
 
@@ -909,7 +918,7 @@ GAR_HD bool u_accelerator_changed(const DevTables &T, const Work &W, bool act, u
   bool sys = tagcheck && !overlay;
   u32 fl = d.flags;
   if (sys && !(fl & ACCD_MANAGED_TRUE)) ch = true;
-  // the owner tag equals resource/ns/name: guaranteed by the index probe that produced `acc` (kind + key compared there)
+  // the owner tag equals resource/ns/name: guaranteed by the value pass that put `acc` on this object's list (kind + key compared there)
   bool th = sys && !ch;
   bool th_eq = u_streq(th, th ? mkstr(A.slab, d.thost) : Str{A.slab, 0}, lb_dns);
   if (th && !th_eq) ch = true;
@@ -955,7 +964,7 @@ GAR_HD bool eg_contains(const DevTables &T, const AccDigest &d, Str lb_arn) {
 //     an untouched one the snapshot's list;
 //   * the accelerator of an earlier GA_CREATE_CHAIN is listed as GAR_PENDING — unless the user tags overwrite a tag the
 //     list call filters on: then nothing the object wrote is listed and the reference creates again.
-GAR_HD void ga_later_step(const DevTables &T, const Work &W, u32 i, u32 kind, Str okey, u64 okh, u32 jb, u32 j, u32 lb, u32 prev_lb, bool pending, OpSink &s, u32 *ev);
+GAR_HD void ga_later_step(const DevTables &T, const Work &W, u32 i, u32 kind, Str okey, u32 jb, u32 j, u32 lb, u32 prev_lb, bool pending, OpSink &s, u32 *ev);
 
 // Written warp-synchronously: every lane of the warp runs the same outer loops (lbIngress index, accelerator of the
 // owner) and the same probe / compare steps under GAR_ANY votes, carrying its own predicates; nothing returns from
@@ -966,7 +975,6 @@ GAR_HD u32 ga_reconcile(const DevTables &T, const Work &W, u32 i, bool valid, Op
   u32 result = GAR_STATUS(GAR_ST_IGNORED, 0, 0);
   u32 dv = 0, kind = 0, jb = 0, nj = 0;
   Str okey{T.o.slab, 0};
-  u64 okh = 0;
   bool ensure = false;
   if (valid) {
     dv = W.derived[i];
@@ -978,10 +986,9 @@ GAR_HD u32 ga_reconcile(const DevTables &T, const Work &W, u32 i, bool valid, Op
         result = GAR_STATUS(GAR_ST_SKIP_NO_LB, 0, 0);
       } else {
         okey = object_key(T, i);
-        okh = W.okey_hash[i];
         if (!(dv & GAR_DV_GA_MANAGED)) {  // cleanup path (rare): runs divergent, no votes inside
-          OwnerIter it = owner_open(W, okh, okey);
-          for (u32 acc; (acc = owner_next(T, W, kind, it)) != GAR_NONE;) put_delete_chain(T, s, i, kind, acc);
+          const OwnRange ar = own_accs(W, i);
+          for (u32 p = ar.pos; p < ar.end; p++) put_delete_chain(T, s, i, kind, W.own[p].row);
           result = GAR_STATUS(GAR_ST_OK, 0, GAR_EV_DELETED);
         } else {
           ensure = true;
@@ -1038,15 +1045,15 @@ GAR_HD u32 ga_reconcile(const DevTables &T, const Work &W, u32 i, bool valid, Op
     // the first iteration that gets here evaluates the snapshot (all lanes together); later ones (rare) evaluate what the
     // object's own earlier ops left behind, scalar
     const bool later = go && prev_lb != GAR_NONE;
-    if (later) ga_later_step(T, W, i, kind, okey, okh, jb, j, lb, prev_lb, pending, s, &ev);
+    if (later) ga_later_step(T, W, i, kind, okey, jb, j, lb, prev_lb, pending, s, &ev);
     go = go && !later;
-    Cursor oc = u_open(W.ix_owner, go, okh);
+    OwnRange oc = go ? own_accs(W, i) : OwnRange{0, 0};
     Str lb_arn = go ? mkstr(A.slab, A.lb_arn[lb]) : Str{A.slab, 0};
     u32 nacc = 0;
     for (;;) {  // accelerators of the owner, in ListAccelerators order
-      u32 acc = u_owner_next(T, W, go && !stop, kind, okey, oc);
-      bool a = acc != GAR_NONE;
+      bool a = go && !stop && oc.pos < oc.end;
       if (!GAR_ANY(a)) break;
+      u32 acc = a ? W.own[oc.pos++].row : GAR_NONE;
       if (a) nacc++;
       AccDigest d;
       d.flags = 0;
@@ -1106,7 +1113,7 @@ GAR_HD u32 ga_reconcile(const DevTables &T, const Work &W, u32 i, bool valid, Op
   return result;
 }
 
-GAR_HD void ga_later_step(const DevTables &T, const Work &W, u32 i, u32 kind, Str okey, u64 okh, u32 jb, u32 j, u32 lb, u32 prev_lb, bool pending, OpSink &s, u32 *ev) {
+GAR_HD void ga_later_step(const DevTables &T, const Work &W, u32 i, u32 kind, Str okey, u32 jb, u32 j, u32 lb, u32 prev_lb, bool pending, OpSink &s, u32 *ev) {
   const gar_actual &A = T.a;
   bool keep_visible, user_thost;
   user_tag_effects(T, W, i, kind, okey, &keep_visible, &user_thost);
@@ -1122,8 +1129,9 @@ GAR_HD void ga_later_step(const DevTables &T, const Work &W, u32 i, u32 kind, St
     if (dns_differs) s.put(GAR_OP_HEAD(GAR_OP_GA_UPDATE_ACCEL, GAR_CTRL_GA, kind), i, j, GAR_PENDING, lb, GAR_NONE);
     if (arn_differs) s.put(GAR_OP_HEAD(GAR_OP_GA_UPDATE_EG, GAR_CTRL_GA, kind), i, j, GAR_PENDING, GAR_PENDING, lb);
   }
-  OwnerIter it = owner_open(W, okh, okey);
-  for (u32 acc; (acc = owner_next(T, W, kind, it)) != GAR_NONE;) {
+  const OwnRange ar = own_accs(W, i);
+  for (u32 p = ar.pos; p < ar.end; p++) {
+    const u32 acc = W.own[p].row;
     if (dns_differs) s.put(GAR_OP_HEAD(GAR_OP_GA_UPDATE_ACCEL, GAR_CTRL_GA, kind), i, j, acc, lb, GAR_NONE);
     const AccDigest d = W.acc_digest[acc];
     // (more than one listener / endpoint group ended the object at its first iteration)
@@ -1146,13 +1154,26 @@ GAR_HD void ga_later_step(const DevTables &T, const Work &W, u32 i, u32 kind, St
 // process{Service,Ingress}CreateOrUpdate of the route53 controller (route53/service.go:48-111, ingress.go:40-104),
 // ensureRoute53 (route53.go:56-130) and CleanupRecordSet (:132-165).
 
-// The owner-value rows of one object key, ascending by value row (= zone-major), fetched ONCE per object.  The
-// first OWNED_CACHE rows are kept in registers/local memory; objects owning more fall back to re-walking the bucket.
-constexpr u32 OWNED_CACHE = 8;
+// The owner-value rows of one owner key, ascending by value row (= zone-major).  Records of both sources carry the value row,
+// a0 = record, a1 = zone (low 30 bits), s1 = record name.
 struct OwnedHit {
   u32 v, rec, zone;
   gar_str name;  // record name of the set that carries the value
 };
+GAR_HD OwnedHit owned_hit(const IdxEntry &e) { return OwnedHit{e.row, e.a0, e.a1 & 0x3FFFFFFFu, e.s1}; }
+// an object in the cache: its canonical row's value segment
+struct OwnedList {
+  const IdxEntry *e;
+  u32 n;
+};
+GAR_HD OwnedList owned_list(const Work &W, u32 i) {
+  const OwnRange r = own_vals(W, i);
+  return OwnedList{W.own + r.pos, r.end - r.pos};
+}
+GAR_HD OwnedHit owned_get(const DevTables &, const Work &, const OwnedList &o, u32 k) { return owned_hit(load_entry(o.e + k)); }
+// a key that left the cache (deleted keys of gar_diff_keys): a walk of ix_val.  The first OWNED_CACHE rows are kept in
+// registers/local memory; keys owning more fall back to re-walking the bucket.
+constexpr u32 OWNED_CACHE = 8;
 struct Owned {
   OwnedHit hit[OWNED_CACHE];
   u32 n;  // total number of owned value rows (may exceed OWNED_CACHE)
@@ -1172,29 +1193,8 @@ GAR_HD void owned_collect(const DevTables &T, const Work &W, u64 okh, u32 kind, 
   IdxEntry e;
   while (idx_next(W.ix_val, c, &e)) {
     if (!owned_match(T, e, kind, key)) continue;
-    if (o.n < OWNED_CACHE) o.hit[o.n] = OwnedHit{e.row, e.a0, e.a1 & 0x3FFFFFFFu, e.s1};
+    if (o.n < OWNED_CACHE) o.hit[o.n] = owned_hit(e);
     o.n++;
-  }
-}
-GAR_HD void u_owned_collect(const DevTables &T, const Work &W, bool active, u64 okh, u32 kind, Str key, Owned &o) {
-  if (active) {
-    o.n = 0;
-    o.okh = okh;
-    o.kind = kind;
-    o.key = key;
-  }
-  Cursor c = active ? idx_open(W.ix_val, okh) : Cursor{0, 0, 0};
-  for (; GAR_ANY(c.pos < c.end);) {
-    IdxEntry e;
-    bool hit = false;
-    if (c.pos < c.end) {
-      e = load_entry(W.ix_val.ent + c.pos++);
-      hit = e.tag == c.tag && (e.a1 >> 31) == kind;
-    }
-    if (u_streq(hit, hit ? mkstr(T.a.slab, e.s0) : Str{T.a.slab, 0}, key)) {
-      if (o.n < OWNED_CACHE) o.hit[o.n] = OwnedHit{e.row, e.a0, e.a1 & 0x3FFFFFFFu, e.s1};
-      o.n++;
-    }
   }
 }
 GAR_HD OwnedHit owned_get(const DevTables &T, const Work &W, const Owned &o, u32 k) {
@@ -1206,7 +1206,7 @@ GAR_HD OwnedHit owned_get(const DevTables &T, const Work &W, const Owned &o, u32
   while (idx_next(W.ix_val, c, &e)) {
     if (!owned_match(T, e, o.kind, o.key)) continue;
     if (seen++ == k) {
-      h = OwnedHit{e.row, e.a0, e.a1 & 0x3FFFFFFFu, e.s1};
+      h = owned_hit(e);
       break;
     }
   }
@@ -1239,7 +1239,8 @@ GAR_HD u32 next_alias_any(const DevTables &T, const Work &W, u32 zone, Str name,
 }
 
 // CleanupRecordSet for one owner key: per zone, owned alias sets in record order, then owner metadata sets
-GAR_HD void r53_cleanup(const DevTables &T, const Work &W, u32 obj, u32 kind, const Owned &ow, OpSink &s) {
+template <class OwnedT>
+GAR_HD void r53_cleanup(const DevTables &T, const Work &W, u32 obj, u32 kind, const OwnedT &ow, OpSink &s) {
   const gar_actual &A = T.a;
   u32 head = GAR_OP_HEAD(GAR_OP_R53_DELETE_RECORD, GAR_CTRL_R53, obj == GAR_NONE ? 0 : kind);
   u32 k = 0;
@@ -1291,20 +1292,15 @@ GAR_HD u32 r53_reconcile(const DevTables &T, const Work &W, u32 i, bool valid, O
   const gar_actual &A = T.a;
   u32 result = GAR_STATUS(GAR_ST_IGNORED, 0, 0);
   u32 kind = 0, jb = 0, nj = 0;
-  Str okey{T.o.slab, 0}, hostnames{T.o.slab, 0};
-  u64 okh = 0;
+  Str hostnames{T.o.slab, 0};
   bool ensure = false;
-  Owned ow;
-  ow.n = 0;
+  OwnedList ow{W.own, 0};
   if (valid) {
     u32 dv = W.derived[i];
     if (dv & GAR_DV_R53_ELIGIBLE) {
       kind = o.obj_kind[i];
-      okey = object_key(T, i);
-      okh = W.okey_hash[i];
       if (!(dv & GAR_DV_R53_ANNOTATED)) {  // cleanup path: divergent, no votes inside
-        owned_collect(T, W, okh, kind, okey, ow);
-        r53_cleanup(T, W, i, kind, ow, s);
+        r53_cleanup(T, W, i, kind, owned_list(W, i), s);
         result = GAR_STATUS(GAR_ST_OK, 0, GAR_EV_DELETED);
       } else {
         ensure = true;
@@ -1315,7 +1311,7 @@ GAR_HD u32 r53_reconcile(const DevTables &T, const Work &W, u32 i, bool valid, O
     }
   }
   u32 ev = 0;
-  bool stop = false, collected = false;
+  bool stop = false;
   // self-observation (include/garecon.h): a hostname this object visited before — earlier in the annotation or at an earlier
   // lbIngress — has its alias record in place, pointing at the accelerator of that visit
   bool have_prev = false;
@@ -1356,10 +1352,7 @@ GAR_HD u32 r53_reconcile(const DevTables &T, const Work &W, u32 i, bool valid, O
       }
     }
     Str acc_dns = go ? mkstr(A.slab, acc_dns_ref) : Str{A.slab, 0};
-    if (GAR_ANY(go && !collected)) {  // the object's owner-value rows, fetched once (all lanes walk their bucket together)
-      u_owned_collect(T, W, go && !collected, okh, kind, okey, ow);
-      if (go) collected = true;
-    }
+    if (go) ow = owned_list(W, i);
     bool created = false;
     u32 pos = 0, k = 0;
     for (;;) {  // hostnames of the annotation, in order: strings.Split(annotation, ",")
@@ -1537,16 +1530,12 @@ GAR_HD void r53_fill_pairs(const DevTables &T, const Work &W, u32 i, u32 t) {
 // warp-synchronous; one lane per (object, hostname)
 GAR_HD void r53_pair(const DevTables &T, const Work &W, u32 p, bool valid) {
   const gar_actual &A = T.a;
-  u32 i = 0, kind = 0;
-  Str hn{T.o.slab, 0}, okey{T.o.slab, 0};
-  u64 okh = 0;
+  u32 i = 0;
+  Str hn{T.o.slab, 0};
   valid = valid && W.pair_code[p] != PAIR_REPEAT;
   if (valid) {
     i = W.pair_obj[p];
     hn = mkstr(T.o.slab, W.pair_hn[p]);
-    kind = T.o.obj_kind[i];
-    okey = object_key(T, i);
-    okh = W.okey_hash[i];
   }
   u32 zone = u_find_hosted_zone(T, W, valid, hn);
   bool live = valid && zone != GAR_NONE;
@@ -1554,26 +1543,22 @@ GAR_HD void r53_pair(const DevTables &T, const Work &W, u32 p, bool valid) {
   // unescapes to hostname + ".", the smallest first-alias-A row (route53.go:216-238,360-367)
   u32 rec = GAR_NONE;
   gar_str rec_alias = 0;
-  Cursor c = u_open(W.ix_val, live, okh);
+  OwnRange c = live ? own_vals(W, i) : OwnRange{0, 0};
   for (; GAR_ANY(c.pos < c.end);) {
     IdxEntry e;
-    bool hit = false;
+    bool mine = false;
     if (c.pos < c.end) {
-      e = load_entry(W.ix_val.ent + c.pos++);
-      hit = e.tag == c.tag && (e.a1 >> 31) == kind && (e.a1 & 0x3FFFFFFFu) == zone;
+      e = load_entry(W.own + c.pos++);
+      mine = (e.a1 & 0x3FFFFFFFu) == zone;
     }
-    bool mine = u_streq(hit, hit ? mkstr(A.slab, e.s0) : Str{A.slab, 0}, okey);
     Str nm = mine ? mkstr(A.slab, e.s1) : Str{A.slab, 0};
     bool plain = mine && !(e.a1 & VALNAME_HAS_BACKSLASH);
     bool shape = plain && nm.n == hn.n + 1 && nm.p[nm.n - 1] == '.';
     bool match = u_streq(shape, substr(nm, 0, shape ? hn.n : 0), hn);
     if (mine && !plain) match = record_name_matches(nm, hn);  // possible \052 escape: scalar, rare
-    if (match) {
-      ValLink l = W.val_link[e.row];
-      if (l.alias_row != GAR_NONE && (rec == GAR_NONE || l.alias_row < rec)) {
-        rec = l.alias_row;
-        rec_alias = l.alias_dns;
-      }
+    if (match && e.tag != GAR_NONE && (rec == GAR_NONE || e.tag < rec)) {  // tag = the value's first alias A record (ValLink)
+      rec = e.tag;
+      rec_alias = e.s0;
     }
   }
   // needRecordsUpdate (route53.go:373-381)
@@ -1622,35 +1607,63 @@ GAR_HD u32 r53_combine(const DevTables &T, const Work &W, u32 i, u32 t, bool val
 
 // ------------------------------------------------------------------ orphans (delete events of keys that left the cache)
 
-GAR_HD bool object_in_cache(const DevTables &T, const Work &W, u32 kind, Str key, u64 key_hash) {
+// the object row with (kind, key), GAR_NONE if the cache has none: the first hit of the ordered ix_obj bucket, i.e. the
+// lowest row with that key (the canonical row, Work::obj_canon)
+GAR_HD u32 find_object(const DevTables &T, const Work &W, u32 kind, Str key, u64 key_hash) {
   Cursor c = idx_open(W.ix_obj, key_hash);
   IdxEntry e;
   while (idx_next(W.ix_obj, c, &e))
-    if (e.a0 == kind && streq(mkstr(T.o.slab, e.s0), key)) return true;
-  return false;
+    if (e.a0 == kind && streq(mkstr(T.o.slab, e.s0), key)) return e.row;
+  return GAR_NONE;
+}
+// Duplicate object keys: rows of an ordered ix_obj bucket (two or more entries, ascending) that repeat the key of an earlier
+// row read the owned lists of the first row with that key.  Every other row keeps obj_canon[i] = i (classify_objects).
+GAR_HD void canon_bucket(const IdxEntry *ent, u32 lo, u32 m, const u8 *oslab, u32 *canon) {
+  for (u32 k = 1; k < m; k++) {
+    const IdxEntry x = ent[lo + k];
+    for (u32 j = 0; j < k; j++) {
+      const IdxEntry y = ent[lo + j];
+      if (y.tag == x.tag && y.a0 == x.a0 && streq(mkstr(oslab, y.s0), mkstr(oslab, x.s0))) {
+        canon[x.row] = y.row;
+        break;
+      }
+    }
+  }
 }
 
 // process{Service,Ingress}Delete of the globalaccelerator controller (service.go:28-52, ingress.go:29-54) for an
 // accelerator whose owner key has no object: returns 1 and emits the delete op
 GAR_HD u32 ga_orphan(const DevTables &T, const Work &W, u32 acc, OpSink &s) {
   if (acc >= W.acc_guest_from) return 0;
-  if (W.acc_claimed && W.acc_claimed[acc]) return 0;  // its owner's object iterated it: the object is in the cache
   u32 fl = W.acc_flags[acc];
   if (!(fl & ACC_MINE) || !(fl & ACC_OWNER_3PART)) return 0;
-  u32 kind = (fl & ACC_OWNER_INGRESS) ? 1u : 0u;
-  if (object_in_cache(T, W, kind, mkstr(T.a.slab, W.acc_owner_key[acc]), W.acc_owner_hash[acc])) return 0;
+  if (W.acc_obj[acc] != GAR_NONE) return 0;  // resolved by the value pass: its object is in the cache
   put_delete_chain(T, s, GAR_NONE, 0, acc);
   return 1;
 }
 
-// is value row v an owner value of this cluster whose object left the cache?
-GAR_HD void mark_orphan_value(const DevTables &T, const Work &W, u32 v) {
-  u32 cls = W.val_cls[v];
-  u8 orphan = 0;
-  if (cls & VAL_OWNER_3PART) {
-    u32 kind = (cls & VAL_OWNER_INGRESS) ? 1u : 0u;
-    orphan = object_in_cache(T, W, kind, mkstr(T.a.slab, W.val_key[v]), W.val_key_hash[v]) ? 0 : 1;
+// The owner-keyed joins, resolved once per snapshot (and after an object delta).  Every owner value is resolved, 3-part key
+// or not: the owner-value match of the reference compares the whole key (owned_match), and an object key may itself hold
+// more than one '/'.  Only 3-part values can be orphans (the controller never writes any other shape).  A resolved row is
+// counted in its object's list segment (own_begin, scanned into the CSR afterwards).
+GAR_HD void resolve_accel(const DevTables &T, const Work &W, u32 a) {
+  const u32 fl = W.acc_flags[a];
+  u32 o = GAR_NONE;
+  if (acc_in_owner_index(W, a, fl)) {
+    o = find_object(T, W, (fl & ACC_OWNER_INGRESS) ? 1u : 0u, mkstr(T.a.slab, W.acc_owner_key[a]), W.acc_owner_hash[a]);
+    if (o != GAR_NONE) GAR_HIST_ADD(&W.own_begin[2 * o]);
   }
+  W.acc_obj[a] = o;
+}
+GAR_HD void resolve_value(const DevTables &T, const Work &W, u32 v) {
+  u32 cls = W.val_cls[v];
+  u32 o = GAR_NONE;
+  if (cls != VAL_NOT_OWNER) {
+    o = find_object(T, W, (cls & VAL_OWNER_INGRESS) ? 1u : 0u, mkstr(T.a.slab, W.val_key[v]), W.val_key_hash[v]);
+    if (o != GAR_NONE) GAR_HIST_ADD(&W.own_begin[2 * o + 1]);
+  }
+  W.val_obj[v] = o;
+  const u8 orphan = (cls & VAL_OWNER_3PART) && o == GAR_NONE ? 1 : 0;
   if (orphan) {
     u32 rec = W.val_rec[v];
     ix_count(W.hist[IX_OVN], key_hash_zoned_h(W.rec_zone[rec], W.rec_name_hash[rec]));
