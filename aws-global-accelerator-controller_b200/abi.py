@@ -497,10 +497,11 @@ class Engine:
         return [(arr[i].name.decode(), float(arr[i].ms), int(arr[i].launches)) for i in range(min(n, 128))]
 
     def counters(self) -> dict:
-        """Exact sizes of the intermediate relations of the last diff (include/garecon.h GAR_CTR_*)."""
+        """Exact sizes of the intermediate relations of the last diff, and how it issued its launches (launch_mode: 0 eager,
+        1 recorded, 2 replayed) (include/garecon.h GAR_CTR_*)."""
         arr = (C.c_uint64 * 8)()
         n = self.lib.gar_last_counters(self._h, arr, 8)
-        names = ("r53_pairs", "dports")
+        names = ("r53_pairs", "dports", "launch_mode")
         return {names[i]: int(arr[i]) for i in range(min(n, len(names)))}
 
     def algorithmic_bytes(self, cs: GarChangeset) -> int:

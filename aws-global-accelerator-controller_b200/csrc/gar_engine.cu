@@ -1319,6 +1319,7 @@ static void do_diff(gar_engine *e, gar_changeset *out, bool to_host, const gar_k
   }
   e->last_counters[GAR_CTR_R53_PAIRS] = P.n_pairs;
   e->last_counters[GAR_CTR_DPORTS] = dc.n_dports;
+  e->last_counters[GAR_CTR_LAUNCH_MODE] = partial ? 0 : (u64)P.last_launch_mode;
   e->last_timings.clear();
   for (auto &m : e->marks) {
     float ms = 0;

@@ -1358,8 +1358,10 @@ struct Pipeline {
   // capacities only grow, so a snapshot shape settles after its first diff.
   // `replayable`: the launch sequence of this flavour depends only on the snapshot and the capacities, so the backend may record
   // it once and replay it (a CUDA graph): the full diff.  Incremental / binding diffs take new host inputs every time.
+  int last_launch_mode = 0;  // graph_begin's answer for the last attempt of the last diff (0 for partial diffs; gar_last_counters)
   template <class DecideF>
   int run_with(DiffCounts *dc, bool full, DecideF decide) {
+    last_launch_mode = 0;
     for (int attempt = 0; attempt < 8; attempt++) {
       u64 sig = 0;
       if (full) {
@@ -1367,6 +1369,7 @@ struct Pipeline {
         sig = hmix(sig, hmix(orphan_sweep ? 5 : 6, tiny_caps ? 7 : 8)) | 1;
       }
       const int g = full ? be.graph_begin(sig) : 0;
+      last_launch_mode = g;
       int rc = GAR_OK;
       if (g != 2) {
         if (!prepared) rc = prepare();

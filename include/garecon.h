@@ -603,7 +603,9 @@ uint32_t gar_last_stage_timings(gar_engine *e, gar_stage_timing *out, uint32_t c
 enum {
   GAR_CTR_R53_PAIRS = 0,   /* (object, route53 hostname) pairs evaluated by the r53_pairs stage (route53.go:84-124 loop bodies) */
   GAR_CTR_DPORTS = 1,      /* ports parsed from listen-ports annotations */
-  GAR_CTR_N = 2
+  GAR_CTR_LAUNCH_MODE = 2, /* how the last diff issued its launches: 0 eager, 1 recorded into a CUDA graph, 2 replayed from one.
+                              Incremental and binding diffs always report 0 */
+  GAR_CTR_N = 3
 };
 uint32_t gar_last_counters(gar_engine *e, uint64_t *out, uint32_t cap);
 

@@ -159,10 +159,14 @@ struct gar_engine {
       run += v;
     }
   }
-  void sort_pairs(u32 *keys, u32 *vals, u32 *, u32 *, u32 n, int) {
+  // stable by the key's low 8 * ceil(bits / 8) bits: exactly what the GPU's 8-bit LSD passes see, so a caller whose keys
+  // exceed its `bits` is wrong here as well
+  void sort_pairs(u32 *keys, u32 *vals, u32 *, u32 *, u32 n, int bits) {
+    const int seen = 8 * ((bits + 7) / 8);
+    const u32 mask = seen >= 32 ? 0xFFFFFFFFu : (1u << seen) - 1u;
     std::vector<u32> idx(n);
     std::iota(idx.begin(), idx.end(), 0u);
-    std::stable_sort(idx.begin(), idx.end(), [&](u32 a, u32 b) { return keys[a] < keys[b]; });
+    std::stable_sort(idx.begin(), idx.end(), [&](u32 a, u32 b) { return (keys[a] & mask) < (keys[b] & mask); });
     std::vector<u32> k(n), v(n);
     for (u32 i = 0; i < n; i++) {
       k[i] = keys[idx[i]];
@@ -385,6 +389,7 @@ uint32_t gar_last_counters(gar_engine *e, uint64_t *out, uint32_t cap) {
   if (!e || !out || cap < GAR_CTR_N) return 0;
   out[GAR_CTR_R53_PAIRS] = e->pipe ? e->pipe->n_pairs : 0;
   out[GAR_CTR_DPORTS] = e->pipe ? e->pipe->n_dports : 0;
+  out[GAR_CTR_LAUNCH_MODE] = 0;  // graph_begin above never records or replays
   return GAR_CTR_N;
 }
 }

@@ -49,13 +49,21 @@ def test_baseline_configs_1e5_bit_exact(garecon, oracle, engine, synth, cfg, n):
     _check_properties(got, snap)
 
 
-@pytest.mark.parametrize("cfg", [3, 5])
-def test_column_major_slabs_1e5_bit_exact(garecon, oracle, engine, synth, cfg):
+@pytest.mark.parametrize("cfg,form", [pytest.param(3, "default", id="3"), pytest.param(5, "default", id="5"),
+                                      pytest.param(3, "no_tma", id="3-no_tma"), pytest.param(3, "tma_all", id="3-tma_all")])
+def test_column_major_slabs_1e5_bit_exact(garecon, oracle, engine, synth, monkeypatch, cfg, form):
     """bench.py's default input layout (every string column contiguous, as host/packer.hpp writes it): same change set as the
-    row-major layout of the same cluster, and equal to the oracle on it."""
+    row-major layout of the same cluster, and equal to the oracle on it.  Config 3 also runs on engines created with
+    GAR_NO_TMA=1 (every staged row pass in its direct-load form) and GAR_TMA_ALL=1 (every one staged)."""
+    from test_backend_kernels import engine_in_form
     snap = synth.generate(cfg, 100_000, layout=1)
-    engine.load(snap)
-    got = engine.diff()
+    if form != "default":
+        with engine_in_form(garecon, monkeypatch, form, cluster_name=snap.cluster) as e:
+            e.load(snap)
+            got = e.diff()
+    else:
+        engine.load(snap)
+        got = engine.diff()
     want = oracle.diff(snap, snap.cluster, mode=1)
     assert got.diff(want) == [], got.describe_first_mismatch(want)
     row = synth.generate(cfg, 100_000)
