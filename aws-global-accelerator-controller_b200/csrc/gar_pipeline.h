@@ -1149,14 +1149,25 @@ struct Pipeline {
     stage1();
     finish_group_a();
   }
-  // a directory shard's tables (gar_shard.h): probes in lbi_*, load balancers, accelerator stubs
+  // a directory shard's tables (gar_shard.h): probes in lbi_*, load balancers, accelerator stubs.  The probes are answered
+  // "first row wins", so every bucket must be in row order: a load-balancer key or target hostname with more rows than
+  // IDX_SMALL_BUCKET (left unordered by the per-bucket ordering) rebuilds both indexes through the stable radix sort, as
+  // prepare() does after a retry.
   void prepare_directory() {
     alloc_work();
+    be.fill32(errflag, 0, FW_WORDS);
     arm_group_a((1u << IX_LB) | (1u << IX_THOST));
     if (T.o.n_lbi) be.for_each("tokenise_hostnames", T.o.n_lbi, FTokenise{T, W});
     if (T.a.n_accels) be.for_each("digest_accelerators", T.a.n_accels, FDigestAccel{T, W});
     if (T.a.n_lbs) be.for_each("hash_load_balancers", T.a.n_lbs, FLbHash{T, W});
     finish_group_a();
+    u32 fl[FW_WORDS];
+    be.download(fl, errflag, sizeof(fl));
+    if (fl[FW_IDX_OVERFLOW]) {
+      u32 *overflow = errflag + FW_IDX_OVERFLOW;
+      W.ix_lb = build_index(S_IX_LB, T.a.n_lbs, 1, FRowLb{T, W}, overflow, true);
+      W.ix_thost = build_index(S_IX_THOST, T.a.n_accels, 1, FRowThost{T, W}, overflow, true);
+    }
   }
 
   u32 dport_cap = 0, pair_cap = 0;  // capacities of the two intermediate relations whose size only the device knows

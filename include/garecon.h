@@ -347,7 +347,14 @@ int gar_snapshot_load(gar_engine *e, const gar_objects *desired, const gar_actua
 
 /* Same, for buffers that already live in device memory of the engine's device (all pointers in the two
    structs are device pointers, the structs themselves are host memory).  No copy is made: the caller keeps
-   the buffers alive until the next load or gar_engine_destroy.  Table validation is skipped. */
+   the buffers alive until the next load or gar_engine_destroy.  Table validation is skipped.
+   What the kernels assume of the caller's buffers (gar_snapshot_load provides the same for its own copies):
+     - each of the two slabs has 32 readable bytes behind slab + slab_len (their values do not matter): string compares
+       and hashes load 8 bytes at a time and the staged row passes copy whole 16-byte lines, both reaching past a string's end;
+     - each slab base is best 16-byte aligned: the staged row passes copy a block's strings to shared memory only from a
+       16-byte aligned slab, otherwise they read every string from the slab directly (same results, slower).  The 8-byte
+       loads are aligned down, so a base that is not 8-byte aligned also has up to 7 bytes before it read;
+     - every column holds its n (begin arrays n + 1) elements at the alignment of its element type, and nothing more. */
 int gar_snapshot_attach_device(gar_engine *e, const gar_objects *desired, const gar_actual *actual);
 
 /* Compute the complete change set for both controllers against the loaded snapshot and copy it to host.

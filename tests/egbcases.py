@@ -83,12 +83,19 @@ def hand_cases():
     return objects, dict(lbs=lbs), bindings, known
 
 
-def random_bindings(seed: int, n_objects: int = 40, n_bindings: int = 120):
+def random_bindings(seed: int, n_objects: int = 40, n_bindings: int = 120, n_known: int = 6, hot: float = 0.0, long: float = 0.0):
+    """n_known endpoint groups, all but the last known to AWS; a fraction `hot` of the bindings all name the first one and a
+    fraction `long` carry 64-191 extra endpoint ids.  Those two draw from a second generator, so that with hot = long = 0 the
+    model is the same as without them."""
     rng = random.Random(seed * 7919 + 13)
+    extra = random.Random(seed * 7919 + 14)
     objects, actual = randmodel.make(seed, n_objects=n_objects)
     lbs = actual.get("lbs", [])
     arns = [lb["arn"] for lb in lbs] + ["arn:stale:1", "arn:stale:2"]
-    known = [EG + str(i) for i in range(6)]
+    first_arn = {}  # (name, region) -> ARN of the first load balancer of that name in that region
+    for lb in lbs:
+        first_arn.setdefault((lb["name"], lb["region"]), lb["arn"])
+    known = [EG + str(i) for i in range(n_known)]
     bindings = []
     for _ in range(n_bindings):
         ob = rng.choice(objects) if objects and rng.random() < 0.9 else None
@@ -104,17 +111,19 @@ def random_bindings(seed: int, n_objects: int = 40, n_bindings: int = 120):
             # start from the object's own load balancers, then perturb
             for h in ob.get("lb_ingress", []):
                 t = pyref.tokenise(h)
-                if t[0] < 3:
-                    for lb in lbs:
-                        if lb["name"] == t[1] and lb["region"] == t[2]:
-                            ids.append(lb["arn"])
-                            break
+                if t[0] < 3 and (t[1], t[2]) in first_arn:
+                    ids.append(first_arn[t[1], t[2]])
             if rng.random() < 0.4 and ids:
                 ids.pop(rng.randrange(len(ids)))
             if rng.random() < 0.3:
                 ids.insert(rng.randrange(len(ids) + 1), rng.choice(arns))
         elif r < 0.85:
             ids = [rng.choice(arns) for _ in range(rng.randrange(0, 5))]
-        bindings.append(dict(ns=ns, ref=ref, eg_arn=rng.choice(known + [EG + "gone"]), deleting=rng.random() < 0.2, finalizers=rng.random() < 0.85,
-                             observed=rng.random() < 0.7, endpoint_ids=ids))
-    return objects, actual, bindings, known[:5]
+        b = dict(ns=ns, ref=ref, eg_arn=rng.choice(known + [EG + "gone"]), deleting=rng.random() < 0.2, finalizers=rng.random() < 0.85,
+                 observed=rng.random() < 0.7, endpoint_ids=ids)
+        if hot and extra.random() < hot:
+            b["eg_arn"] = known[0]
+        if long and extra.random() < long:
+            b["endpoint_ids"] = ids + [extra.choice(arns) for _ in range(extra.randrange(64, 192))]
+        bindings.append(b)
+    return objects, actual, bindings, known[:-1]

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 import randmodel
+import scalemodels
 
 
 def _pick(objects, actual, rng):
@@ -71,6 +72,26 @@ def test_hostsim_keys_match_oracle_and_full_diff(garecon, oracle, hostsim, seed)
     assert inc.diff(want) == [], inc.describe_first_mismatch(want)
     assert inc2.diff(want) == []
     assert full.diff(oracle.diff(snap, "default", mode=1)) == []
+    _check_against_full(inc, full, rows)
+
+
+def test_hostsim_dropped_objects(garecon, oracle, hostsim):
+    """A 2000-object randmodel cluster with 8 % of its objects dropped after generation: their accelerators, TXT owner values and
+    alias records are orphans (randmodel alone makes 0-3 at any size).  Full diff, and a shuffled 10 % batch with the dropped
+    keys (and keys that match nothing) as deleted keys."""
+    objects, actual, dropped = scalemodels.randmodel_dropped(2, 2000)
+    snap = garecon.pack(objects, actual)
+    hostsim.load(snap)
+    full = hostsim.diff()
+    want = oracle.diff(snap, "default", mode=1)
+    assert full.diff(want) == [], full.describe_first_mismatch(want)
+    sb = [int(x) for x in want.section_begin]
+    assert len(dropped) > 100 and sb[2] - sb[1] > 50 and sb[4] - sb[3] > 200
+    rows = random.Random(2).sample(range(len(objects)), len(objects) // 10)
+    deleted = dropped + scalemodels.ABSENT_KEYS
+    inc = hostsim.diff_keys(rows, deleted)
+    want = oracle.diff_keys(snap, rows, deleted, mode=1)
+    assert inc.diff(want) == [], inc.describe_first_mismatch(want)
     _check_against_full(inc, full, rows)
 
 
