@@ -152,6 +152,13 @@ class ActualDeltaResult(tuple):
             raise AttributeError(name) from None
 
 
+COMPACT_OBJECTS, COMPACT_ACTUAL = 1, 2
+
+
+class GarCompactResult(C.Structure):
+    _fields_ = [(k, C.c_uint64) for k in ("obj_slab_before", "obj_slab_len", "act_slab_before", "act_slab_len")]
+
+
 EGB_DELETING, EGB_HAS_FINALIZERS, EGB_OBSERVED = 1, 2, 4
 (OP_EGB_ADD_FINALIZER, OP_EGB_REMOVE_FINALIZER, OP_EGB_REMOVE_ENDPOINT, OP_EGB_ADD_ENDPOINT, OP_EGB_UPDATE_WEIGHT, OP_EGB_UPDATE_STATUS) = range(11, 17)
 ST_REQUEUE_1S = 8
@@ -304,6 +311,10 @@ def load_library(path: os.PathLike | None = None) -> C.CDLL:
     lib.gar_snapshot_apply_objects.restype = C.c_int
     lib.gar_snapshot_apply_actual.argtypes = [C.c_void_p, C.POINTER(GarActualDelta), C.POINTER(GarActualDeltaResult)]
     lib.gar_snapshot_apply_actual.restype = C.c_int
+    lib.gar_snapshot_compact.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(GarCompactResult)]
+    lib.gar_snapshot_compact.restype = C.c_int
+    lib.gar_snapshot_read_slab.argtypes = [C.c_void_p, C.c_uint32, C.c_uint64, C.c_uint64, C.c_void_p]
+    lib.gar_snapshot_read_slab.restype = C.c_int
     lib.gar_shard_route.argtypes = [C.c_void_p, C.POINTER(GarShard), C.c_int, _u64p, _u64p]
     lib.gar_shard_route.restype = C.c_int
     lib.gar_shard_pack.argtypes = [C.c_void_p, C.c_void_p]
@@ -337,7 +348,7 @@ def load_library(path: os.PathLike | None = None) -> C.CDLL:
 
 EXPORTED_SYMBOLS = (
     "gar_engine_create", "gar_engine_destroy", "gar_snapshot_load", "gar_snapshot_attach_device", "gar_diff",
-    "gar_diff_device", "gar_diff_keys", "gar_bindings_diff", "gar_snapshot_apply_objects", "gar_snapshot_apply_actual", "gar_shard_route", "gar_shard_pack", "gar_shard_unpack", "gar_shard_blob_bytes",
+    "gar_diff_device", "gar_diff_keys", "gar_bindings_diff", "gar_snapshot_apply_objects", "gar_snapshot_apply_actual", "gar_snapshot_compact", "gar_snapshot_read_slab", "gar_shard_route", "gar_shard_pack", "gar_shard_unpack", "gar_shard_blob_bytes",
     "gar_shard_arena", "gar_shard_open_peers", "gar_shard_pack_peers",
     "gar_changeset_free", "gar_last_error", "gar_version", "gar_algorithmic_bytes",
     "gar_last_stage_timings", "gar_last_counters",
@@ -425,6 +436,20 @@ class Engine:
         res = GarActualDeltaResult()
         self._check(self.lib.gar_snapshot_apply_actual(self._h, C.byref(d), C.byref(res)))
         return ActualDeltaResult(res)
+
+    def compact(self, groups: int = COMPACT_OBJECTS | COMPACT_ACTUAL) -> GarCompactResult:
+        """Rebuild the resident slabs of `groups` (COMPACT_OBJECTS | COMPACT_ACTUAL) dense on the device (include/garecon.h
+        gar_snapshot_compact).  -> the slab lengths before and after."""
+        res = GarCompactResult()
+        self._check(self.lib.gar_snapshot_compact(self._h, int(groups), C.byref(res)))
+        return res
+
+    def read_slab(self, group: int, off: int, length: int) -> np.ndarray:
+        """`length` bytes at `off` of the resident slab of `group` (COMPACT_OBJECTS or COMPACT_ACTUAL) as a uint8 array
+        (include/garecon.h gar_snapshot_read_slab): how tok_name / tok_region of a change set are resolved."""
+        buf = np.zeros(max(1, int(length)), dtype=np.uint8)
+        self._check(self.lib.gar_snapshot_read_slab(self._h, int(group), int(off), int(length), buf.ctypes.data_as(C.c_void_p)))
+        return buf[:int(length)]
 
     def bindings_diff(self, bindings) -> ChangeSet:
         """EndpointGroupBinding set-diff against the loaded snapshot; `bindings` has a .struct (GarBindings)."""

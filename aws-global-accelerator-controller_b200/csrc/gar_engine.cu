@@ -25,6 +25,7 @@
 #include "gar_pipeline.h"
 #include "gar_shard.h"
 #include "gar_delta.h"
+#include "gar_compact.h"
 
 #define GAR_VERSION_STRING "garecon 0.1.0 (sm_90a)"
 
@@ -177,36 +178,38 @@ __global__ void k_fill32(u32 *p, u32 v, size_t n) {
   for (; i < n; i += stride) p[i] = v;
 }
 
-// ---- exclusive scan (u32): per-tile reduce, single-block scan of tile sums, per-tile scan + offset
+// ---- exclusive scan (u32 counts; u64 byte offsets of the slab compaction): per-tile reduce, single-block scan of tile sums, per-tile scan + offset
 constexpr int SCAN_THREADS = 256;
 constexpr int SCAN_ITEMS = 8;
 constexpr int SCAN_TILE = SCAN_THREADS * SCAN_ITEMS;
 
-__device__ __forceinline__ u32 warp_incl_scan(u32 v) {
+template <class V>
+__device__ __forceinline__ V warp_incl_scan(V v) {
   const unsigned lane = threadIdx.x & 31;
 #pragma unroll
   for (int d = 1; d < 32; d <<= 1) {
-    u32 t = __shfl_up_sync(0xffffffffu, v, d);
+    V t = __shfl_up_sync(0xffffffffu, v, d);
     if (lane >= (unsigned)d) v += t;
   }
   return v;
 }
 // exclusive scan of one value per thread across the block; returns the exclusive prefix, *total = block sum
-__device__ __forceinline__ u32 block_excl_scan(u32 v, u32 *total) {
-  __shared__ u32 wsum[SCAN_THREADS / 32];
-  __shared__ u32 wtot;
+template <class V>
+__device__ __forceinline__ V block_excl_scan(V v, V *total) {
+  __shared__ V wsum[SCAN_THREADS / 32];
+  __shared__ V wtot;
   const unsigned lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  u32 inc = warp_incl_scan(v);
+  V inc = warp_incl_scan(v);
   if (lane == 31) wsum[w] = inc;
   __syncthreads();
   if (w == 0) {
-    u32 s = lane < SCAN_THREADS / 32 ? wsum[lane] : 0;
-    u32 si = warp_incl_scan(s);
+    V s = lane < SCAN_THREADS / 32 ? wsum[lane] : 0;
+    V si = warp_incl_scan(s);
     if (lane < SCAN_THREADS / 32) wsum[lane] = si - s;
     if (lane == SCAN_THREADS / 32 - 1) wtot = si;
   }
   __syncthreads();
-  u32 r = wsum[w] + inc - v;
+  V r = wsum[w] + inc - v;
   *total = wtot;
   __syncthreads();
   return r;
@@ -215,42 +218,53 @@ __device__ __forceinline__ u32 block_excl_scan(u32 v, u32 *total) {
 // Single-pass chained scan with decoupled look-back.  Tiles take a ticket (so a tile only ever waits on tiles that
 // already run or ran), publish their aggregate, then their inclusive prefix; a tile's exclusive prefix is the sum
 // of its predecessors' aggregates back to the first published inclusive prefix.
-// state word: bits 62..63 = 0 empty, 1 aggregate, 2 inclusive prefix; low 32 bits = value.
-__global__ void __launch_bounds__(SCAN_THREADS) k_scan_lookback(u32 *data, u32 n, unsigned long long *state, u32 *ticket) {
-  __shared__ u32 s_tile, s_excl;
+// state word: bits 62..63 = 0 empty, 1 aggregate, 2 inclusive prefix; the bits below = value (u32 sums wrap as u32 does; u64 sums
+// are slab offsets, below 2^40).
+constexpr unsigned long long SCAN_VALUE = (1ull << 62) - 1;
+template <class V>
+__global__ void __launch_bounds__(SCAN_THREADS) k_scan_lookback(V *data, u32 n, unsigned long long *state, u32 *ticket) {
+  constexpr int PER16 = 16 / sizeof(V);  // elements per 16-byte access
+  __shared__ u32 s_tile;
+  __shared__ V s_excl;
   if (threadIdx.x == 0) s_tile = atomicAdd(ticket, 1u);
   __syncthreads();
   const u32 tile = s_tile;
   const u32 base = tile * SCAN_TILE + threadIdx.x * SCAN_ITEMS;
-  u32 v[SCAN_ITEMS];
+  V v[SCAN_ITEMS];
   if (base + SCAN_ITEMS <= n) {
     const uint4 *q = reinterpret_cast<const uint4 *>(data + base);
-    uint4 a = q[0], b = q[1];
-    v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w;
-    v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+#pragma unroll
+    for (int k = 0; k < SCAN_ITEMS / PER16; k++) {
+      const uint4 a = q[k];
+      if constexpr (sizeof(V) == 4) {
+        v[4 * k] = a.x; v[4 * k + 1] = a.y; v[4 * k + 2] = a.z; v[4 * k + 3] = a.w;
+      } else {
+        v[2 * k] = (V)a.x | ((V)a.y << 32); v[2 * k + 1] = (V)a.z | ((V)a.w << 32);
+      }
+    }
   } else {
 #pragma unroll
     for (int k = 0; k < SCAN_ITEMS; k++) v[k] = base + k < n ? data[base + k] : 0;
   }
-  u32 s = 0;
+  V s = 0;
 #pragma unroll
   for (int k = 0; k < SCAN_ITEMS; k++) s += v[k];
-  u32 total;
-  u32 ex = block_excl_scan(s, &total);
+  V total;
+  V ex = block_excl_scan(s, &total);
   if (threadIdx.x < 32) {  // warp 0 looks back over 32 predecessors per step
     volatile unsigned long long *st = state;
     const unsigned lane = threadIdx.x;
     if (tile == 0) {
       if (lane == 0) {
-        st[0] = (2ull << 62) | total;
+        st[0] = (2ull << 62) | (unsigned long long)total;
         s_excl = 0;
       }
     } else {
       if (lane == 0) {
-        st[tile] = (1ull << 62) | total;
+        st[tile] = (1ull << 62) | (unsigned long long)total;
         __threadfence();
       }
-      u32 excl = 0;
+      V excl = 0;
       for (long long p = (long long)tile - 1;; p -= 32) {
         long long idx = p - (long long)lane;
         unsigned long long w = 2ull << 62;  // before tile 0: an inclusive prefix of 0
@@ -261,14 +275,14 @@ __global__ void __launch_bounds__(SCAN_THREADS) k_scan_lookback(u32 *data, u32 n
         }
         unsigned pm = __ballot_sync(0xffffffffu, (w >> 62) == 2);
         int first = __ffs(pm) - 1;  // nearest predecessor that already knows its inclusive prefix
-        u32 val = (first < 0 || (int)lane <= first) ? (u32)w : 0u;
+        V val = (first < 0 || (int)lane <= first) ? (V)(w & SCAN_VALUE) : (V)0;
 #pragma unroll
         for (int off = 16; off > 0; off >>= 1) val += __shfl_down_sync(0xffffffffu, val, off);
         excl += val;  // meaningful in lane 0
         if (first >= 0) break;
       }
       if (lane == 0) {
-        st[tile] = (2ull << 62) | (u32)(excl + total);
+        st[tile] = (2ull << 62) | (unsigned long long)(V)(excl + total);
         s_excl = excl;
       }
     }
@@ -276,18 +290,21 @@ __global__ void __launch_bounds__(SCAN_THREADS) k_scan_lookback(u32 *data, u32 n
   __syncthreads();
   ex += s_excl;
   if (base + SCAN_ITEMS <= n) {
-    uint4 a, b;
-    a.x = ex; ex += v[0];
-    a.y = ex; ex += v[1];
-    a.z = ex; ex += v[2];
-    a.w = ex; ex += v[3];
-    b.x = ex; ex += v[4];
-    b.y = ex; ex += v[5];
-    b.z = ex; ex += v[6];
-    b.w = ex;
     uint4 *q = reinterpret_cast<uint4 *>(data + base);
-    q[0] = a;
-    q[1] = b;
+#pragma unroll
+    for (int k = 0; k < SCAN_ITEMS / PER16; k++) {
+      uint4 a;
+      if constexpr (sizeof(V) == 4) {
+        a.x = ex; ex += v[4 * k];
+        a.y = ex; ex += v[4 * k + 1];
+        a.z = ex; ex += v[4 * k + 2];
+        a.w = ex; ex += v[4 * k + 3];
+      } else {
+        a.x = (u32)ex; a.y = (u32)(ex >> 32); ex += v[2 * k];
+        a.z = (u32)ex; a.w = (u32)(ex >> 32); ex += v[2 * k + 1];
+      }
+      q[k] = a;
+    }
   } else {
 #pragma unroll
     for (int k = 0; k < SCAN_ITEMS; k++) {
@@ -450,6 +467,9 @@ struct InvalidError {
 struct StateError {
   std::string msg;
 };
+struct DeviceMemoryError {
+  std::string msg;
+};
 
 static std::string g_create_error = "";
 
@@ -495,6 +515,104 @@ __global__ void __launch_bounds__(256) k_shard_pack_rows(const __grid_constant__
       bulk_s2g(dst + head, t + head, body);
       asm volatile("cp.async.bulk.commit_group;" ::: "memory");
       asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // the tile must stay until it has been read
+    }
+  }
+}
+
+// ---- slab compaction (gar_compact.h step 3): the copy of the live strings into the new slab, output-centric.  A block owns one
+// window of COMPACT_WINDOW destination bytes, finds the strings that overlap it by binary search in the new offsets and
+// assembles the window in shared memory: each warp takes 32 strings at a time (references and offsets in one coalesced load per
+// lane), then copies them one after the other with all lanes, so both the slab loads and the shared-memory stores are
+// contiguous; sources are near-contiguous wherever the old layout was column-major.  One thread then writes the window with a
+// bulk store (cp.async.bulk.global.shared::cta, as k_shard_pack_rows does).  Windows start at multiples of 16 bytes of a
+// 16-byte aligned slab, so only the last window has a tail that goes out by ordinary stores.  No warp loops over more than
+// COMPACT_LONG bytes of one string: longer strings are left out here and copied by k_compact_long, launched behind this kernel.
+__global__ void __launch_bounds__(256) k_compact_copy(u8 *__restrict__ dst, const u8 *__restrict__ src, const gar_str *__restrict__ sref,
+                                                      const u64 *__restrict__ off, u32 m, u64 total) {
+  __shared__ alignas(128) u8 tile[COMPACT_WINDOW];
+  __shared__ u32 s_p[2];
+  const u64 lo = (u64)blockIdx.x * COMPACT_WINDOW, hi = min(lo + COMPACT_WINDOW, total);
+  if (threadIdx.x == 0) s_p[0] = compact_first(off, m, lo);
+  if (threadIdx.x == 32) s_p[1] = compact_end(off, m, hi);
+  __syncthreads();
+  const u32 p0 = s_p[0], p1 = s_p[1];
+  if (p1 - p0 == 1 && GAR_STR_LEN(sref[p0]) > COMPACT_LONG) return;  // the inside of a long string: nothing to assemble
+  const u32 lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (u32 b = p0 + warp * 32; b < p1; b += 256) {
+    const u32 p = b + lane;
+    gar_str r = 0;
+    u64 o = 0;
+    if (p < p1) {
+      r = sref[p];
+      o = off[p];
+    }
+    u32 len = GAR_STR_LEN(r);
+    if (len > COMPACT_LONG) len = 0;
+    const u64 a = max(o, lo), e = min(o + len, hi);
+    const u32 cnt = e > a ? (u32)(e - a) : 0u, at = (u32)(a - lo);
+    const u64 from = GAR_STR_OFF(r) + (a - o);
+    unsigned live = __ballot_sync(0xffffffffu, cnt != 0);
+    while (live) {
+      const int j = __ffs(live) - 1;
+      live &= live - 1;
+      const u8 *sp = src + __shfl_sync(0xffffffffu, from, j);
+      const u32 c = __shfl_sync(0xffffffffu, cnt, j);
+      u8 *tp = tile + __shfl_sync(0xffffffffu, at, j);
+      for (u32 k = lane; k < c; k += 32) tp[k] = sp[k];
+    }
+  }
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // the tile was written through the generic proxy, the bulk store reads it through the async one
+  __syncthreads();
+  const u32 bytes = (u32)(hi - lo), body = bytes & ~15u;
+  if (threadIdx.x == 0 && body) {
+    bulk_s2g(dst + lo, tile, body);
+    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // the tile must stay until it has been read
+  }
+  if (threadIdx.x >= 32 && threadIdx.x - 32 < bytes - body) dst[lo + body + threadIdx.x - 32] = tile[body + threadIdx.x - 32];
+}
+// Strings longer than COMPACT_LONG, same windows: the block lists the long strings that overlap its window (at most
+// COMPACT_WINDOW / COMPACT_LONG + 2) and copies the part of each that falls inside with all 256 threads, 16 bytes per thread and
+// step: a string of several MiB is spread over as many blocks as it has windows.  Destination-aligned 16-byte stores; a source
+// at another phase is read as two aligned 16-byte loads and shifted (it may over-read up to 31 bytes: GAR_SLAB_PAD); the
+// unaligned head and tail of the part go by bytes.
+constexpr u32 COMPACT_LONG_LIST = COMPACT_WINDOW / COMPACT_LONG + 2;
+__global__ void __launch_bounds__(256) k_compact_long(u8 *__restrict__ dst, const u8 *__restrict__ src, const gar_str *__restrict__ sref,
+                                                      const u64 *__restrict__ off, u32 m, u64 total) {
+  __shared__ u32 s_p[2], s_n, s_list[COMPACT_LONG_LIST];
+  const u64 lo = (u64)blockIdx.x * COMPACT_WINDOW, hi = min(lo + COMPACT_WINDOW, total);
+  if (threadIdx.x == 0) {
+    s_p[0] = compact_first(off, m, lo);
+    s_n = 0;
+  }
+  if (threadIdx.x == 32) s_p[1] = compact_end(off, m, hi);
+  __syncthreads();
+  const u32 p0 = s_p[0], p1 = s_p[1];
+  for (u32 p = p0 + threadIdx.x; p < p1; p += 256)
+    if (GAR_STR_LEN(sref[p]) > COMPACT_LONG) s_list[atomicAdd(&s_n, 1u)] = p;
+  __syncthreads();
+  for (u32 q = 0; q < s_n; q++) {
+    const u32 p = s_list[q];
+    const gar_str r = sref[p];
+    const u64 o = off[p], a = max(o, lo), e = min(o + GAR_STR_LEN(r), hi);
+    u8 *d = dst + a;
+    const u8 *f = src + GAR_STR_OFF(r) + (a - o);
+    const u32 n = (u32)(e - a), head = min(n, (u32)((16 - ((uintptr_t)d & 15)) & 15)), body = (n - head) >> 4, tail = n - head - 16 * body;
+    if (threadIdx.x < head) d[threadIdx.x] = f[threadIdx.x];
+    if (threadIdx.x >= 32 && threadIdx.x - 32 < tail) d[head + 16 * body + threadIdx.x - 32] = f[head + 16 * body + threadIdx.x - 32];
+    const u32 sh = (u32)((uintptr_t)(f + head) & 15), bits = (sh & 7) * 8;
+    const uint4 *fa = (const uint4 *)(f + head - sh);
+    uint4 *da = (uint4 *)(d + head);
+    for (u32 k = threadIdx.x; k < body; k += 256) {
+      uint4 x = fa[k];
+      if (sh) {
+        const uint4 y = fa[k + 1];
+        const u64 q0 = (u64)x.x | ((u64)x.y << 32), q1 = (u64)x.z | ((u64)x.w << 32), q2 = (u64)y.x | ((u64)y.y << 32), q3 = (u64)y.z | ((u64)y.w << 32);
+        const u64 w0 = sh < 8 ? q0 : q1, w1 = sh < 8 ? q1 : q2, w2 = sh < 8 ? q2 : q3;
+        const u64 l = bits ? (w0 >> bits) | (w1 << (64 - bits)) : w0, h = bits ? (w1 >> bits) | (w2 << (64 - bits)) : w1;
+        x = make_uint4((u32)l, (u32)(l >> 32), (u32)h, (u32)(h >> 32));
+      }
+      da[k] = x;
     }
   }
 }
@@ -794,14 +912,17 @@ struct gar_engine {
   void copy32(u32 *dst, const u32 *src, size_t n) {
     if (n) CK(cudaMemcpyAsync(dst, src, n * 4, cudaMemcpyDeviceToDevice, stream));
   }
-  void exclusive_scan(u32 *data, u32 n) {
+  void exclusive_scan(u32 *data, u32 n) { scan(data, n); }
+  void exclusive_scan(u64 *data, u32 n) { scan(data, n); }
+  template <class V>
+  void scan(V *data, u32 n) {
     if (!n) return;
     stage_begin("exclusive_scan");
     u32 ntiles = (n + SCAN_TILE - 1) / SCAN_TILE;
     size_t sbytes = 8 * (size_t)(ntiles + 2);
     unsigned long long *state = (unsigned long long *)dev_ensure(d_scan_tiles, sbytes);
     CK(cudaMemsetAsync(state, 0, sbytes, stream));  // tile states + the ticket counter (last word)
-    k_scan_lookback<<<ntiles, SCAN_THREADS, 0, stream>>>(data, n, state, (u32 *)(state + ntiles + 1));
+    k_scan_lookback<V><<<ntiles, SCAN_THREADS, 0, stream>>>(data, n, state, (u32 *)(state + ntiles + 1));
     launches += 1;
     stage_end();
   }
@@ -887,6 +1008,40 @@ struct gar_engine {
       b.cap = want;
     }
     return (u8 *)b.p;
+  }
+
+  // ---- slab compaction (gar_compact.h): group g's new slab waits in compact_new[g] until the standby columns are swapped in
+  DBuf compact_new[CG_N];
+  DBuf &resident_slab(int g) { return in[g == CG_OBJECTS ? DC_N : DC_N + 1 + AC_N]; }
+  u8 *compact_slab(int g, u64 bytes) {
+    DBuf &b = compact_new[g];
+    const size_t want = ((size_t)bytes + 255) & ~(size_t)255;
+    if (cudaMalloc(&b.p, want) != cudaSuccess) {
+      cudaGetLastError();
+      b.p = nullptr;
+      return nullptr;
+    }
+    b.cap = want;
+    return (u8 *)b.p;
+  }
+  void compact_slab_commit(int g, bool keep) {
+    DBuf &b = compact_new[g];
+    CK(cudaStreamSynchronize(stream));  // the copy kernels read the old slab
+    if (keep) std::swap(b, resident_slab(g));
+    CK(cudaFree(b.p));
+    b = DBuf{};
+  }
+  void compact_copy(u8 *dst, const u8 *src, const gar_str *sref, const u64 *off, u32 m, u64 total, bool any_long) {
+    if (!total) return;
+    const u32 windows = (u32)((total + COMPACT_WINDOW - 1) / COMPACT_WINDOW);
+    stage_begin("compact_copy");
+    k_compact_copy<<<windows, 256, 0, stream>>>(dst, src, sref, off, m, total);
+    launches++;
+    if (any_long) {
+      k_compact_long<<<windows, 256, 0, stream>>>(dst, src, sref, off, m, total);
+      launches++;
+    }
+    stage_end();
   }
 };
 
@@ -1160,6 +1315,58 @@ static void do_apply_actual(gar_engine *e, const gar_actual_delta *d, gar_actual
   }
 }
 
+
+// ------------------------------------------------------------------ slab compaction
+
+static void do_compact(gar_engine *e, u32 groups, gar_compact_result *out) {
+  if (!groups || (groups & ~(u32)(GAR_COMPACT_OBJECTS | GAR_COMPACT_ACTUAL))) throw InvalidError{"groups must be a non-empty mask of GAR_COMPACT_OBJECTS | GAR_COMPACT_ACTUAL"};
+  if (!e->loaded) throw StateError{"no snapshot loaded"};
+  if (e->attached) throw StateError{"compaction needs a snapshot the engine owns: an attached (device) snapshot cannot be changed"};
+  if (e->shard_home || e->shard_round != 0) throw StateError{"compaction is not available in sharded mode"};
+  CK(cudaSetDevice(e->device));
+  e->graph_drop();
+  e->marks.clear();
+  e->events_used = 0;
+  e->stage_depth = 0;
+  try {
+    Compactor<gar_engine> C{*e, e->T};
+    const int rc = C.run(groups, *out);
+    CK(cudaStreamSynchronize(e->stream));
+    CK(cudaGetLastError());
+    for (int g = 0; g < CG_N; g++)  // the per-string staging arrays are as large as the reference columns: not kept
+      for (DBuf *b : {&e->dscratch[CS_SREF + g], &e->dscratch[CS_OFF + g]}) {
+        CK(cudaFree(b->p));
+        *b = DBuf{};
+      }
+    if (rc == GAR_E_NOMEM) throw DeviceMemoryError{C.error};
+    if (rc != GAR_OK) throw InvalidError{C.error};
+    e->slice = e->T;
+    if (e->pipe) {
+      e->pipe->T = e->T;
+      if (groups & GAR_COMPACT_OBJECTS) e->pipe->obj_stale = true;  // as after an object delta: the object side is rebuilt by the next diff
+      if (groups & GAR_COMPACT_ACTUAL) e->pipe->prepared = false;   // as after an AWS delta
+    }
+    e->input_bytes = table_bytes(&e->T.o, &e->T.a);
+  } catch (const CudaError &) {
+    e->loaded = false;  // the compaction may have stopped half-way: no snapshot until the next load
+    delete e->pipe;
+    e->pipe = nullptr;
+    throw;
+  }
+}
+
+static void do_read_slab(gar_engine *e, u32 group, u64 off, u64 len, void *dst) {
+  if (group != GAR_COMPACT_OBJECTS && group != GAR_COMPACT_ACTUAL) throw InvalidError{"group must be GAR_COMPACT_OBJECTS or GAR_COMPACT_ACTUAL"};
+  if (!e->loaded) throw StateError{"no snapshot loaded"};
+  if (e->shard_home) throw StateError{"a sharded sub-snapshot's strings live in the receive buffers"};
+  const u8 *slab = group == GAR_COMPACT_OBJECTS ? e->T.o.slab : e->T.a.slab;
+  const u64 slab_len = group == GAR_COMPACT_OBJECTS ? e->T.o.slab_len : e->T.a.slab_len;
+  if (off > slab_len || len > slab_len - off) throw InvalidError{"off + len beyond the resident slab_len"};
+  if (len && !dst) throw InvalidError{"NULL destination"};
+  CK(cudaSetDevice(e->device));
+  if (len) e->download(dst, slab + off, len);
+}
+
 static void do_diff(gar_engine *e, gar_changeset *out, bool to_host, const gar_keyset *ks = nullptr, const gar_bindings *bd = nullptr) {
   if (!e->loaded) throw InvalidError{"no snapshot loaded"};
   CK(cudaSetDevice(e->device));
@@ -1362,6 +1569,9 @@ static int guarded(gar_engine *e, Fn fn) {
   } catch (const StateError &se) {
     e->err = se.msg;
     return GAR_E_STATE;
+  } catch (const DeviceMemoryError &me) {
+    e->err = me.msg;
+    return GAR_E_NOMEM;
   } catch (const std::bad_alloc &) {
     e->err = "out of host memory";
     return GAR_E_NOMEM;
@@ -1442,6 +1652,7 @@ void gar_engine_destroy(gar_engine *e) {
   for (auto &b : e->dset) cudaFree(b.p);
   for (auto &b : e->dscratch) cudaFree(b.p);
   for (auto &b : e->aset) cudaFree(b.p);
+  for (auto &b : e->compact_new) cudaFree(b.p);
   cudaFree(e->d_valid.p);
   for (int k = 0; k < 2; k++) {
     if (e->dl_pin[k].p) cudaFreeHost(e->dl_pin[k].p);
@@ -1517,6 +1728,15 @@ int gar_snapshot_apply_objects(gar_engine *e, const gar_object_delta *d, gar_del
 int gar_snapshot_apply_actual(gar_engine *e, const gar_actual_delta *d, gar_actual_delta_result *out) {
   if (!d || !out) return GAR_E_INVALID;
   return guarded(e, [&] { do_apply_actual(e, d, out); });
+}
+
+int gar_snapshot_compact(gar_engine *e, uint32_t groups, gar_compact_result *out) {
+  if (!out) return GAR_E_INVALID;
+  return guarded(e, [&] { do_compact(e, groups, out); });
+}
+
+int gar_snapshot_read_slab(gar_engine *e, uint32_t group, uint64_t off, uint64_t len, void *dst) {
+  return guarded(e, [&] { do_read_slab(e, group, off, len, dst); });
 }
 
 int gar_shard_route(gar_engine *e, const gar_shard *shard, int round, uint64_t *meta, uint64_t *send_bytes) {

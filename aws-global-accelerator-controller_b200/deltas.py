@@ -166,6 +166,12 @@ class ColumnMirror:
         self.cur["slab"] = np.asarray(both["slab"])
         return np.array(up_row, dtype=np.uint32), np.array(del_row, dtype=np.uint32), np.array(moved, dtype=np.uint32)
 
+    def compact(self) -> int:
+        """The mirror of gar_snapshot_compact(GAR_COMPACT_OBJECTS): the slab holds exactly the live strings.  -> slab_len."""
+        self.cur = compact(self.cur)
+        self.slab_len = len(self.cur["slab"])
+        return self.slab_len
+
     def snapshot(self, a_cols: dict) -> "tables.Snapshot":
         """A loadable snapshot of the mirrored object table with the given AWS tables."""
         return tables.from_columns(self.cur, a_cols)
@@ -321,6 +327,12 @@ class ActualMirror:
         out["slab_base"] = base
         out["slab_len"] = self.slab_len
         return out
+
+    def compact(self) -> int:
+        """The mirror of gar_snapshot_compact(GAR_COMPACT_ACTUAL): the slab holds exactly the live strings.  -> slab_len."""
+        self.cur = compact_actual(self.cur)
+        self.slab_len = len(self.cur["slab"])
+        return self.slab_len
 
     def snapshot(self, o_cols: dict) -> "tables.Snapshot":
         """A loadable snapshot of the given object table with the mirrored AWS tables."""

@@ -401,8 +401,8 @@ int gar_diff_keys(gar_engine *e, const gar_keyset *keys, gar_changeset *out);
    The table stays dense (object row order has no meaning: informer List order is unspecified), so every later call sees a
    table exactly like the one a gar_snapshot_load of the same objects would give, with two exceptions that the change set
    shows: tok_name / tok_region reference the resident object slab, where the strings of delta k sit at its slab_base.
-   The resident object slab is append-only: strings of replaced and deleted rows stay until the next gar_snapshot_load;
-   slab_len tells the caller when a reload is worth it.
+   The resident object slab is append-only: strings of replaced and deleted rows stay until gar_snapshot_compact (below) drops
+   them; slab_len tells the caller when a compaction is worth it.
    Atomic: the upsert table passes the checks of gar_snapshot_load (string references inside its own slab, monotone CSRs,
    kind / spec-type range, the ns/name layout rule) and the key rule above before anything resident changes; on
    GAR_E_INVALID the snapshot is unchanged.  A CUDA error in the middle leaves no loaded snapshot: later deltas return
@@ -445,7 +445,7 @@ int gar_snapshot_apply_objects(gar_engine *e, const gar_object_delta *d, gar_del
        size, zone_target entries are distinct, and delta zone k's zone_name equals resident zone zone_target[k]'s name byte
        for byte; otherwise GAR_E_INVALID;
      - the strings of `rows` are appended to the resident AWS slab at a 16-byte aligned slab_base (append-only, as for
-       objects; slab_len tells the caller when a reload is worth it).
+       objects; slab_len tells the caller when a gar_snapshot_compact is worth it).
    Atomic: `rows` passes the checks gar_snapshot_load applies to an actual table (enums, monotone CSRs, strings inside its
    slab), and the rules above hold, before anything resident changes; on GAR_E_INVALID the snapshot is unchanged.  GAR_E_STATE
    in the same cases as gar_snapshot_apply_objects; after a CUDA error in the middle no snapshot is loaded.  Every later gar_diff,
@@ -471,6 +471,49 @@ typedef struct gar_actual_delta_result {
   uint64_t slab_len;               /* resident AWS slab bytes after the delta, strings of replaced rows included */
 } gar_actual_delta_result;
 int gar_snapshot_apply_actual(gar_engine *e, const gar_actual_delta *d, gar_actual_delta_result *out);
+
+/* ---------------------------------------------------------------- slab compaction: dropping the dead strings on the device
+   Deltas only append to the two resident slabs.  gar_snapshot_compact rebuilds the slab of each selected group (`groups`: a
+   mask of GAR_COMPACT_*) so that it holds exactly the strings the resident columns reference, entirely on the device: no byte
+   comes from the host, and a worker that keeps its snapshot current by deltas needs neither a reload nor a host copy of the
+   tables to get rid of the growth.
+   Layout after the call (part of the contract: a caller can mirror it; deltas.compact / deltas.compact_actual of the Python
+   package state it in numpy).  Per group, for each gar_str column in struct declaration order, the strings of rows 0 .. n-1
+   back to back, no separators, no padding between strings or columns; slab_len is the sum of the live lengths.
+     - objects: the key column comes first.  obj_ns[i] and obj_name[i] are slices of one "ns/name" string: the key is copied
+       once, len(ns) + 1 + len(name) bytes from obj_ns[i]'s offset, and both references point into the copy (there is no
+       separate name column).  Then obj_ingress_class, ann_key, ann_val, lbi_hostname, port_proto.
+     - AWS: lb_region, lb_name, lb_dns, lb_arn, acc_name, acc_dns, tag_key, tag_val, ep_id, zone_name, rec_name, rec_alias_dns,
+       val_value.
+     - obj_ingress_class on a row without GAR_OBJ_HAS_INGRESS_CLASS, and rec_alias_dns on a row with rec_has_alias == 0, count as
+       empty: whatever the reference held is not read (it may point outside the slab) and is replaced by an empty one.
+     - an empty string keeps length 0 and gets the running offset of its column.
+     - strings are never shared afterwards: two references to the same bytes become two copies (only the key pair stays
+       shared).  For a hand-packed table that interned strings slab_len may therefore grow; `out` reports it, it is no error.
+     - row order, every CSR and every fixed-width column are untouched.  The slab keeps GAR_SLAB_PAD zero bytes behind slab_len.
+   Every later gar_diff, gar_diff_device, gar_diff_keys, gar_bindings_diff, gar_snapshot_apply_objects and
+   gar_snapshot_apply_actual answers bit for bit as before the call, except that tok_name / tok_region reference the new object
+   slab (equal as the strings they name; gar_snapshot_read_slab resolves them) and later deltas report slab_base / slab_len
+   relative to the compacted slab.
+   groups == 0 or unknown bits: GAR_E_INVALID.  GAR_E_STATE in exactly the cases of gar_snapshot_apply_objects.  The new slabs and
+   the rewritten reference columns are built in standby buffers and become resident together after the last kernel was queued: if
+   a new slab cannot be allocated the call returns GAR_E_NOMEM and the snapshot is unchanged and usable (GAR_E_INVALID the same
+   way if un-sharing would push a slab past 2^40 bytes); a CUDA error in the middle leaves no loaded snapshot, as for the deltas.
+   The old slabs' memory is released.  Compacting the object group leaves the engine as an object delta does (the object side is
+   rebuilt by the next diff, the AWS side stays prepared); compacting the AWS group drops the prepared state as an AWS delta
+   does.  Both drop the recorded launch sequence. */
+enum { GAR_COMPACT_OBJECTS = 1u << 0, GAR_COMPACT_ACTUAL = 1u << 1 };
+typedef struct gar_compact_result {
+  uint64_t obj_slab_before, obj_slab_len;   /* resident object slab bytes before / after (equal when not selected) */
+  uint64_t act_slab_before, act_slab_len;   /* the same for the AWS slab */
+} gar_compact_result;
+int gar_snapshot_compact(gar_engine *e, uint32_t groups, gar_compact_result *out);
+
+/* Copies `len` bytes at `off` of a resident slab to host memory (group = GAR_COMPACT_OBJECTS or GAR_COMPACT_ACTUAL, exactly one):
+   how a caller reads the strings tok_name / tok_region name without mirroring the slab itself.  off + len beyond the resident
+   slab_len, or a group that is not exactly one of the two: GAR_E_INVALID.  GAR_E_STATE before a load and on a sharded
+   sub-snapshot (its strings live in the receive buffers). */
+int gar_snapshot_read_slab(gar_engine *e, uint32_t group, uint64_t off, uint64_t len, void *dst);
 
 /* ---------------------------------------------------------------- EndpointGroupBinding set-diff (SURVEY.md §8 row f3)
    The third controller's decisions (pkg/controller/endpointgroupbinding/reconcile.go:20-217): finalizer handling and the
