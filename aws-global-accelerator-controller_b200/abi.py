@@ -152,6 +152,20 @@ class ActualDeltaResult(tuple):
             raise AttributeError(name) from None
 
 
+class GarZoneDelta(C.Structure):
+    _fields_ = [("added", C.POINTER(GarActual)), ("added_at", _u32p), ("n_deleted", C.c_uint32), ("deleted", _u32p)]
+
+
+class GarZoneDeltaResult(C.Structure):
+    _fields_ = [("n_zones", C.c_uint32), ("n_records", C.c_uint32), ("n_values", C.c_uint32), ("slab_base", C.c_uint64), ("slab_len", C.c_uint64)]
+
+
+class ZoneDeltaResult(ActualDeltaResult):
+    """Outcome of one zone delta (include/garecon.h gar_zone_delta_result): n_zones, n_records, n_values, slab_base, slab_len."""
+    __slots__ = ()
+    FIELDS = ("n_zones", "n_records", "n_values", "slab_base", "slab_len")
+
+
 COMPACT_OBJECTS, COMPACT_ACTUAL = 1, 2
 
 
@@ -311,6 +325,8 @@ def load_library(path: os.PathLike | None = None) -> C.CDLL:
     lib.gar_snapshot_apply_objects.restype = C.c_int
     lib.gar_snapshot_apply_actual.argtypes = [C.c_void_p, C.POINTER(GarActualDelta), C.POINTER(GarActualDeltaResult)]
     lib.gar_snapshot_apply_actual.restype = C.c_int
+    lib.gar_snapshot_apply_zones.argtypes = [C.c_void_p, C.POINTER(GarZoneDelta), C.POINTER(GarZoneDeltaResult)]
+    lib.gar_snapshot_apply_zones.restype = C.c_int
     lib.gar_snapshot_compact.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(GarCompactResult)]
     lib.gar_snapshot_compact.restype = C.c_int
     lib.gar_snapshot_read_slab.argtypes = [C.c_void_p, C.c_uint32, C.c_uint64, C.c_uint64, C.c_void_p]
@@ -348,7 +364,7 @@ def load_library(path: os.PathLike | None = None) -> C.CDLL:
 
 EXPORTED_SYMBOLS = (
     "gar_engine_create", "gar_engine_destroy", "gar_snapshot_load", "gar_snapshot_attach_device", "gar_diff",
-    "gar_diff_device", "gar_diff_keys", "gar_bindings_diff", "gar_snapshot_apply_objects", "gar_snapshot_apply_actual", "gar_snapshot_compact", "gar_snapshot_read_slab", "gar_shard_route", "gar_shard_pack", "gar_shard_unpack", "gar_shard_blob_bytes",
+    "gar_diff_device", "gar_diff_keys", "gar_bindings_diff", "gar_snapshot_apply_objects", "gar_snapshot_apply_actual", "gar_snapshot_apply_zones", "gar_snapshot_compact", "gar_snapshot_read_slab", "gar_shard_route", "gar_shard_pack", "gar_shard_unpack", "gar_shard_blob_bytes",
     "gar_shard_arena", "gar_shard_open_peers", "gar_shard_pack_peers",
     "gar_changeset_free", "gar_last_error", "gar_version", "gar_algorithmic_bytes",
     "gar_last_stage_timings", "gar_last_counters",
@@ -436,6 +452,17 @@ class Engine:
         res = GarActualDeltaResult()
         self._check(self.lib.gar_snapshot_apply_actual(self._h, C.byref(d), C.byref(res)))
         return ActualDeltaResult(res)
+
+    def apply_zones(self, added: GarActual | None = None, added_at=(), deleted=()) -> ZoneDeltaResult:
+        """Zone delta against the loaded snapshot (include/garecon.h gar_snapshot_apply_zones).  `added`: a GarActual holding only
+        new hosted zones with their record lists, e.g. tables.pack([], {"zones": [...]}).actual (its buffers must stay alive for
+        the call); added_at[k]: the resident zone row new zone k is listed in front of (n_zones: behind the last), non-decreasing;
+        `deleted`: resident zone rows removed with their records."""
+        at, dl = (np.ascontiguousarray(np.asarray(list(v), dtype=np.uint32).reshape(-1)) for v in (added_at, deleted))
+        d = GarZoneDelta(C.pointer(added) if added is not None else None, at.ctypes.data_as(_u32p), len(dl), dl.ctypes.data_as(_u32p))
+        res = GarZoneDeltaResult()
+        self._check(self.lib.gar_snapshot_apply_zones(self._h, C.byref(d), C.byref(res)))
+        return ZoneDeltaResult(res)
 
     def compact(self, groups: int = COMPACT_OBJECTS | COMPACT_ACTUAL) -> GarCompactResult:
         """Rebuild the resident slabs of `groups` (COMPACT_OBJECTS | COMPACT_ACTUAL) dense on the device (include/garecon.h

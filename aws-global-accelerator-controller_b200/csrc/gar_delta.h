@@ -25,7 +25,9 @@
 //
 // AWS deltas (gar_snapshot_apply_actual, ActualSplicer below) re-lay only the AWS families a delta touches — load balancers;
 // accelerator -> tag / listener -> port range / listener -> endpoint group -> endpoint; zone -> record -> value — with one
-// generic step per parent -> child link, order preserving.  They drop the whole prepared state (the caller does).
+// generic step per parent -> child link, order preserving.  They drop the whole prepared state (the caller does).  Zone
+// deltas (gar_snapshot_apply_zones) run on the same splicer: a source map of the zone table with deletes and positioned
+// inserts (FDeltaZoneMap), then the same re-layout of zone -> record -> value, zone names included.
 #pragma once
 
 #include <stddef.h>
@@ -258,6 +260,34 @@ struct FDeltaZoneName {
   u32 *bad;
   GAR_HD void operator()(u32 k) const {
     if (!streq(mkstr(rslab, rname[target[k]]), mkstr(dslab, dname[k]))) *bad = 1;
+  }
+};
+// #{m : a[m] < x} for a ascending
+GAR_HD u32 delta_rank(const u32 *a, u32 n, u32 x) {
+  u32 lo = 0, hi = n;
+  while (lo < hi) {
+    const u32 mid = (lo + hi) >> 1;
+    if (a[mid] < x) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+// source map of the zone table after a zone delta (include/garecon.h "zone deltas"): thread r < n places resident zone r
+// unless it is deleted, thread n + k new zone k, each at the row the header's formula gives.  del: the deleted rows
+// ascending; at: added_at (non-decreasing)
+struct FDeltaZoneMap {
+  const u32 *del, *at;
+  u32 nd, na, n;
+  u32 *src;
+  GAR_HD void operator()(u32 t) const {
+    if (t < n) {
+      const u32 d = delta_rank(del, nd, t);
+      if (d < nd && del[d] == t) return;
+      src[t - d + delta_rank(at, na, t + 1)] = t;
+    } else {
+      const u32 k = t - n, a = at[k];
+      src[a - delta_rank(del, nd, a) + k] = SRC_UPSERT | k;
+    }
   }
 };
 
@@ -599,13 +629,11 @@ struct ActualSplicer {
   gar_actual R{}, U{}, N{};  // resident table, delta rows (device copies), the table being built
   u64 base = 0;
   bool written[AC_N] = {};
+  bool move_zones = false;  // a zone delta: zone rows move, so zone_name is re-laid with the record lists
 
   // GAR_OK, GAR_E_INVALID (error says why; nothing changed) or another gar_rc
   int apply(const gar_actual_delta &d, gar_actual_delta_result &out) {
-    static const u32 kZero[1] = {0};
-    gar_actual no_rows{};  // an empty table: every CSR is {0}
-    for (int c = 0; c < AC_N; c++)
-      if (kActualCols[c].child != AT_N) actual_col(no_rows, c) = kZero;
+    const gar_actual no_rows = empty_table();
     const gar_actual &H = d.rows ? *d.rows : no_rows;
     R = T.a;
     error = delta_check_actual(H);
@@ -635,21 +663,7 @@ struct ActualSplicer {
     N = R;
     const bool lbs = H.n_lbs || d.n_lb_deleted, accs = H.n_accels || d.n_acc_deleted;
     if (lbs || accs || H.n_zones) {
-      // the delta rows on the device; their strings behind the resident ones
-      U = H;
-      for (int c = 0; c < AC_N; c++) {
-        const ActualColInfo &ci = kActualCols[c];
-        const size_t n = (size_t)actual_rows(H, ci.table) + (ci.child != AT_N ? 1 : 0);
-        actual_col(U, c) = up(DS_A_UP + c, actual_col(H, c), n * ci.width);
-      }
-      if (has_rows) {
-        u8 *slab = be.delta_actual_slab(R.slab_len, base + H.slab_len + GAR_SLAB_PAD);
-        static const u8 kZeros[GAR_SLAB_PAD] = {};
-        if (H.slab_len) be.upload(slab + base, H.slab, H.slab_len);
-        be.upload(slab + base + H.slab_len, kZeros, GAR_SLAB_PAD);
-        T.a.slab = N.slab = slab;  // the resident bytes moved with a grown slab; slab_len changes only with the rest
-        N.slab_len = base + H.slab_len;
-      }
+      stage(H, has_rows);
       int rc = GAR_OK;
       if (lbs) rc = relayout(AT_LB, root_map(AT_LB, n_lbs, lb_key, lb_pairs), n_lbs);
       if (rc == GAR_OK && accs) rc = relayout(AT_ACC, root_map(AT_ACC, n_accels, acc_key, acc_pairs), n_accels);
@@ -673,6 +687,55 @@ struct ActualSplicer {
     return GAR_OK;
   }
 
+  // the zone-set splice of include/garecon.h "zone deltas": the host checks the delta, FDeltaZoneMap writes the zone table's
+  // source map, and relayout() re-lays zone -> record -> value.  GAR_OK, GAR_E_INVALID (error says why; nothing changed) or
+  // another gar_rc
+  int apply(const gar_zone_delta &d, gar_zone_delta_result &out) {
+    const gar_actual no_rows = empty_table();
+    const gar_actual &H = d.added ? *d.added : no_rows;
+    R = T.a;
+    if (H.n_lbs || H.n_accels || H.n_tags || H.n_listeners || H.n_port_ranges || H.n_egs || H.n_endpoints)
+      return invalid("added: a zone delta carries hosted zones and their records only, no load balancer or accelerator rows");
+    error = delta_check_actual(H);
+    if (!error.empty()) return GAR_E_INVALID;
+    const u32 n = R.n_zones, na = H.n_zones, nd = d.n_deleted;
+    if ((na && !d.added_at) || (nd && !d.deleted)) return invalid("NULL added_at or deleted array");
+    for (u32 k = 0; k < na; k++) {
+      if (d.added_at[k] > n) return invalid("added_at out of range");
+      if (k && d.added_at[k] < d.added_at[k - 1]) return invalid("added_at decreases");
+    }
+    std::vector<u32> del(d.deleted, d.deleted + nd);
+    std::sort(del.begin(), del.end());
+    for (u32 m = 0; m < nd; m++) {
+      if (del[m] >= n) return invalid("deleted zone row out of range");
+      if (m && del[m] == del[m - 1]) return invalid("a zone row appears twice in deleted");
+    }
+    if ((u64)n - nd + na >= (1u << 27)) return invalid("too many zones for one snapshot");
+    const u32 n_new = n - nd + na;
+    base = na ? (R.slab_len + 15) & ~(u64)15 : 0;
+    if (na && base + H.slab_len + GAR_SLAB_PAD >= (1ull << GAR_STR_OFF_BITS)) return invalid("the resident AWS slab would outgrow 2^40 bytes");
+    N = R;
+    if (na || nd) {
+      stage(H, na != 0);
+      u32 *src = (u32 *)be.delta_scratch(DS_A_SRC + AT_ZONE, 4 * (size_t)(n_new + 1));
+      if (n + na)
+        be.for_each("delta_zone_map", n + na,
+                    FDeltaZoneMap{(const u32 *)up(DS_A_DEL + AT_ZONE, del.data(), 4 * (size_t)nd), (const u32 *)up(DS_A_PAIRS + AT_ZONE, d.added_at, 4 * (size_t)na), nd, na, n, src});
+      move_zones = true;
+      const int rc = relayout(AT_ZONE, src, n_new);
+      if (rc != GAR_OK) return rc;
+      for (int c = 0; c < AC_N; c++)
+        if (written[c]) be.delta_actual_swap(c);
+      T.a = N;
+    }
+    out.n_zones = T.a.n_zones;
+    out.n_records = T.a.n_records;
+    out.n_values = T.a.n_values;
+    out.slab_base = base;
+    out.slab_len = T.a.slab_len;
+    return GAR_OK;
+  }
+
  private:
   int invalid(const std::string &msg) {
     error = msg;
@@ -682,6 +745,31 @@ struct ActualSplicer {
     void *p = be.delta_scratch(k, bytes + GAR_SLAB_PAD + 16);
     if (bytes) be.upload(p, host, bytes);
     return p;
+  }
+  // an empty table: every CSR is {0}
+  static gar_actual empty_table() {
+    static const u32 kZero[1] = {0};
+    gar_actual a{};
+    for (int c = 0; c < AC_N; c++)
+      if (kActualCols[c].child != AT_N) actual_col(a, c) = kZero;
+    return a;
+  }
+  // the delta rows on the device (U); with append_slab their strings go behind the resident ones at `base`
+  void stage(const gar_actual &H, bool append_slab) {
+    U = H;
+    for (int c = 0; c < AC_N; c++) {
+      const ActualColInfo &ci = kActualCols[c];
+      const size_t n = (size_t)actual_rows(H, ci.table) + (ci.child != AT_N ? 1 : 0);
+      actual_col(U, c) = up(DS_A_UP + c, actual_col(H, c), n * ci.width);
+    }
+    if (append_slab) {
+      u8 *slab = be.delta_actual_slab(R.slab_len, base + H.slab_len + GAR_SLAB_PAD);
+      static const u8 kZeros[GAR_SLAB_PAD] = {};
+      if (H.slab_len) be.upload(slab + base, H.slab, H.slab_len);
+      be.upload(slab + base + H.slab_len, kZeros, GAR_SLAB_PAD);
+      T.a.slab = N.slab = slab;  // the resident bytes moved with a grown slab; slab_len changes only with the rest
+      N.slab_len = base + H.slab_len;
+    }
   }
   void *standby(int c, size_t bytes) {
     written[c] = true;
@@ -756,7 +844,7 @@ struct ActualSplicer {
     FDeltaGather g{src, base, 0, {}};
     for (int c = 0; c < AC_N; c++) {
       const ActualColInfo &ci = kActualCols[c];
-      if (ci.table != t || ci.child != AT_N || c == AC_ZONE_NAME) continue;  // zone rows never move: only their record lists change
+      if (ci.table != t || ci.child != AT_N || (c == AC_ZONE_NAME && !move_zones)) continue;  // an AWS delta keeps every zone row in place
       g.c[g.ncols++] = DeltaGatherCol{(const u8 *)actual_col(R, c), (const u8 *)actual_col(U, c), (u8 *)standby(c, (size_t)n * ci.width), ci.width, ci.str};
     }
     if (g.ncols && n) be.for_each("delta_gather", n, g);

@@ -1285,7 +1285,9 @@ static void do_apply(gar_engine *e, const gar_object_delta *d, gar_delta_result 
   }
 }
 
-static void do_apply_actual(gar_engine *e, const gar_actual_delta *d, gar_actual_delta_result *out) {
+// AWS deltas and zone deltas (gar_actual_delta / gar_zone_delta): the same splicer, state checks and prepared-state drop
+template <class Delta, class Result>
+static void do_apply_actual(gar_engine *e, const Delta *d, Result *out) {
   if (!e->loaded) throw StateError{"no snapshot loaded"};
   if (e->attached) throw StateError{"AWS deltas need a snapshot the engine owns: an attached (device) snapshot cannot be changed"};
   if (e->shard_home || e->shard_round != 0) throw StateError{"AWS deltas are not available in sharded mode"};
@@ -1726,6 +1728,11 @@ int gar_snapshot_apply_objects(gar_engine *e, const gar_object_delta *d, gar_del
 }
 
 int gar_snapshot_apply_actual(gar_engine *e, const gar_actual_delta *d, gar_actual_delta_result *out) {
+  if (!d || !out) return GAR_E_INVALID;
+  return guarded(e, [&] { do_apply_actual(e, d, out); });
+}
+
+int gar_snapshot_apply_zones(gar_engine *e, const gar_zone_delta *d, gar_zone_delta_result *out) {
   if (!d || !out) return GAR_E_INVALID;
   return guarded(e, [&] { do_apply_actual(e, d, out); });
 }

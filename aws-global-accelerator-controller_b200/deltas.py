@@ -328,6 +328,39 @@ class ActualMirror:
         out["slab_len"] = self.slab_len
         return out
 
+    def apply_zones(self, added: dict | None = None, added_at=(), deleted=()) -> dict:
+        """The rule of include/garecon.h "zone deltas": for r = 0 .. n_zones, first the new zones with added_at == r in delta
+        order, then resident zone r unless it is deleted; records and values follow their zones.  added: an actual column dict
+        of zones with their records (own slab, no LB or accelerator rows), or None.  -> the result of the delta: n_zones,
+        n_records, n_values, slab_base, slab_len."""
+        cur = self.cur
+        n = len(cur["zone_name"])
+        na = len(added["zone_name"]) if added is not None else 0
+        at = np.asarray(added_at, dtype=np.int64).reshape(-1)
+        gone = set(np.asarray(deleted, dtype=np.int64).reshape(-1).tolist())
+        base, both = 0, cur
+        if na:
+            padded = _pad16(cur)
+            base = len(padded["slab"])
+            both = tables.concat_cols(tables.ACT_TABLES, ["rec", "val"], [padded, added])
+            zb = np.asarray(cur["zone_rec_begin"]).astype(np.int64)
+            both["zone_name"] = np.concatenate([cur["zone_name"], np.asarray(added["zone_name"], dtype=np.uint64) + np.uint64(base)])
+            both["zone_rec_begin"] = np.concatenate([zb, np.asarray(added["zone_rec_begin"]).astype(np.int64)[1:] + zb[-1]]).astype(np.uint32)
+        sel, k = [], 0
+        for r in range(n + 1):
+            while k < na and at[k] == r:
+                sel.append(n + k)
+                k += 1
+            if r < n and r not in gone:
+                sel.append(r)
+        new = {c: v for c, v in cur.items() if c != "slab"}
+        take_tree(both, "zone", np.asarray(sel, dtype=np.int64), new)
+        new["slab"] = np.asarray(both["slab"])
+        self.cur = new
+        self.slab_len = len(new["slab"])
+        s = self.sizes()
+        return {"n_zones": s["n_zones"], "n_records": s["n_records"], "n_values": s["n_values"], "slab_base": base, "slab_len": self.slab_len}
+
     def compact(self) -> int:
         """The mirror of gar_snapshot_compact(GAR_COMPACT_ACTUAL): the slab holds exactly the live strings.  -> slab_len."""
         self.cur = compact_actual(self.cur)
@@ -389,6 +422,66 @@ def aws_churn(mirror: ActualMirror, rng: np.random.Generator, frac: float = 0.01
                 lb_target=np.concatenate([lb_upd, np.full(len(lb_add), GAR_NONE)]).astype(np.uint32),
                 acc_target=np.concatenate([acc_upd, np.full(len(acc_add), GAR_NONE)]).astype(np.uint32),
                 zone_target=zones.astype(np.uint32), lb_deleted=lb_del.astype(np.uint32), acc_deleted=acc_del.astype(np.uint32))
+
+
+def zone_churn(mirror: ActualMirror, rng: np.random.Generator, n_add: int = 10, rec_frac: float = 0.01, n_del: int = 0, serial: int = 0):
+    """One change of the hosted-zone set, as a worker sees it between two ListHostedZones answers: `n_del` random zones deleted
+    and `n_add` zones created at random rows, whose record sets total about `rec_frac` of all records.  With n_add >= 2, the
+    first new zone is a subzone of the zone with the most records, named after one of its record names and holding that
+    name's record sets (so the hostname resolves to the subzone from now on), and the second repeats the name of a resident
+    zone, listed in front of it (so it wins the zone walk), with half of that zone's records.  The others get fresh names and
+    a run of records copied from a random record row on (across zone boundaries).  -> keyword arguments of Engine.apply_zones / ActualMirror.apply_zones, with
+    added = a compact actual column dict."""
+    cur = mirror.cur
+    slab = np.asarray(cur["slab"])
+    n = len(cur["zone_name"])
+    zb = np.asarray(cur["zone_rec_begin"]).astype(np.int64)
+    n_rec = int(zb[-1])
+    budget = int(n_rec * rec_frac)
+    recs, names, at = [], [], []  # per new zone: record rows of `cur`, zone name (gar_str into cur's slab, or fresh bytes), row
+    if n_add >= 2 and n and n_rec:
+        z = int(np.argmax(zb[1:] - zb[:-1]))
+        r = int(rng.integers(zb[z], zb[z + 1]))
+        nm = slab[int(_off(cur["rec_name"][r:r + 1])[0]):][:int(_len(cur["rec_name"][r:r + 1])[0])].tobytes()
+        recs.append(zb[z] + np.flatnonzero(key_is(np.asarray(cur["rec_name"][zb[z]:zb[z + 1]]), slab, nm)))
+        names.append(cur["rec_name"][r])
+        at.append(int(rng.integers(0, n + 1)))
+        d = int(rng.integers(0, n))
+        recs.append(np.arange(zb[d], zb[d] + min((zb[d + 1] - zb[d]) // 2, max(0, budget // 3))))
+        names.append(cur["zone_name"][d])
+        at.append(d)
+    left = max(0, budget - sum(len(x) for x in recs))
+    n_fresh = n_add - len(recs)
+    for i in range(n_fresh):
+        take = min(n_rec, left // n_fresh + (1 if i < left % n_fresh else 0))
+        lo = int(rng.integers(0, n_rec - take + 1))
+        recs.append(np.arange(lo, lo + take))  # a run of record rows, across zone boundaries
+        names.append(b"zc%d-%d.churn.test." % (serial, i))
+        at.append(int(rng.integers(0, n + 1)))
+    order = np.argsort(np.asarray(at, dtype=np.int64), kind="stable")
+    rows = actual_rows(cur)
+    rec_rows = np.concatenate([recs[k] for k in order]).astype(np.int64) if len(order) else np.zeros(0, dtype=np.int64)
+    rows.update(take_tree(cur, "rec", rec_rows))
+    rows["zone_rec_begin"] = np.concatenate([[0], np.cumsum([len(recs[k]) for k in order])]).astype(np.uint32)
+    rows["zone_name"] = np.asarray([0 if isinstance(names[k], bytes) else names[k] for k in order], dtype=np.uint64)
+    added = compact_actual(rows)
+    fresh = [(i, names[k]) for i, k in enumerate(order) if isinstance(names[k], bytes)]
+    if fresh:
+        pos = len(added["slab"])
+        for i, nm in fresh:
+            added["zone_name"][i] = np.uint64(pos) | (np.uint64(len(nm)) << np.uint64(40))
+            pos += len(nm)
+        added["slab"] = np.concatenate([added["slab"], np.frombuffer(b"".join(nm for _, nm in fresh), dtype=np.uint8)])
+    deleted = np.sort(rng.choice(n, size=min(n, n_del), replace=False)) if n_del and n else np.zeros(0, dtype=np.int64)
+    return dict(added=added, added_at=np.asarray(at, dtype=np.uint32)[order], deleted=deleted.astype(np.uint32))
+
+
+def largest_zones_deleted(mirror: ActualMirror, k: int = 10):
+    """A zone delta that deletes the `k` zones with the most records.  -> keyword arguments of Engine.apply_zones /
+    ActualMirror.apply_zones (added = None)."""
+    zb = np.asarray(mirror.cur["zone_rec_begin"]).astype(np.int64)
+    rows = np.sort(np.argsort(-(zb[1:] - zb[:-1]), kind="stable")[:k])
+    return dict(added=None, added_at=np.zeros(0, dtype=np.uint32), deleted=rows.astype(np.uint32))
 
 
 def actual_struct(cols: dict):

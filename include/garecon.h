@@ -434,7 +434,7 @@ int gar_snapshot_apply_objects(gar_engine *e, const gar_object_delta *d, gar_del
      accelerator     DescribeAccelerator + ListTagsForResource + ListListeners + ListEndpointGroups: the whole subtree
                      (tags, listeners, port ranges, endpoint groups, endpoints)          addressed by resident accelerator row
      hosted zone     ListResourceRecordSets(zone): the zone's complete record list        addressed by resident zone row
-   (Adding or removing hosted zones is a reload.)  Rules:
+   (Hosted zones are added and removed by gar_snapshot_apply_zones, below.)  Rules:
      - order preserving: list order is part of the contract (the first (region, name) LB row wins, an owner's accelerators
        are visited in list order, the first matching alias in a zone wins).  Deleted LB and accelerator rows are removed and
        the survivors keep their relative order; a replaced row keeps its position; appended rows follow in delta order.  The
@@ -472,6 +472,44 @@ typedef struct gar_actual_delta_result {
 } gar_actual_delta_result;
 int gar_snapshot_apply_actual(gar_engine *e, const gar_actual_delta *d, gar_actual_delta_result *out);
 
+/* ---------------------------------------------------------------- zone deltas: hosted zones added and removed
+   A changed ListHostedZones answer applied to the loaded zone table on the device, with the record sets of the zones it adds
+   and removes, so that a CreateHostedZone or DeleteHostedZone needs no reload (and no re-list of everything else).  Zone order
+   is part of the contract: the zone walk takes the first row whose name matches, a public and a private zone may share a name,
+   and a new subzone changes the zone of every hostname below it.  Rules:
+     - new order: for r = 0 .. n_zones (the resident count), first the new zones with added_at == r in delta order, then
+       resident zone r unless it is deleted.  So surviving resident row r becomes
+         r - #{deleted rows < r} + #{k : added_at[k] <= r},
+       and new zone k gets row
+         added_at[k] - #{deleted rows < added_at[k]} + k.
+       Records and values follow their zones exactly as a gar_snapshot_load of the resulting tables would lay them out;
+     - duplicate zone names are allowed (the first row wins, as after a load).  Zones cannot be renamed;
+     - the strings of `added` are appended to the resident AWS slab at a 16-byte aligned slab_base, as for
+       gar_snapshot_apply_actual; slab_base is 0 when nothing is added.  A later gar_snapshot_compact lays zone_name out in row
+       order, as always.
+   GAR_E_INVALID, with the snapshot unchanged: a deleted row >= n_zones or deleted twice; added_at[k] > n_zones or added_at
+   decreasing; `added` holding load balancers, accelerators or any of their children; a NULL array with a non-zero count;
+   anything gar_snapshot_load rejects in an actual table.  GAR_E_STATE in the cases of gar_snapshot_apply_actual (before a load,
+   on an attached snapshot, once gar_shard_route has run on the loaded slice, on a sharded sub-snapshot).  After a CUDA error in
+   the middle no snapshot is loaded.  Every later gar_diff, gar_diff_device, gar_diff_keys, gar_bindings_diff, object or AWS
+   delta and compaction answers bit for bit as after a gar_snapshot_load of the same object table and the resulting AWS tables
+   (tok_* reference the resident object slab, as after any delta).  The call drops the prepared state and the recorded launch
+   sequence, as an AWS delta does. */
+typedef struct gar_zone_delta {
+  const gar_actual *added;      /* new hosted zones with their record lists, packed like a load's actual table with its own slab:
+                                   n_zones, zone_name, zone_rec_begin, records, values.  Every other table is empty (n_lbs =
+                                   n_accels = 0, CSRs {0}).  NULL or n_zones == 0: nothing added */
+  const uint32_t *added_at;     /* [added->n_zones] resident zone row that new zone k is listed in front of; the resident n_zones =
+                                   behind the last zone.  Non-decreasing in k */
+  uint32_t n_deleted;
+  const uint32_t *deleted;      /* [n_deleted] resident zone rows, removed together with their record sets; distinct */
+} gar_zone_delta;
+typedef struct gar_zone_delta_result {
+  uint32_t n_zones, n_records, n_values;  /* after the delta */
+  uint64_t slab_base, slab_len;           /* as in gar_actual_delta_result */
+} gar_zone_delta_result;
+int gar_snapshot_apply_zones(gar_engine *e, const gar_zone_delta *d, gar_zone_delta_result *out);
+
 /* ---------------------------------------------------------------- slab compaction: dropping the dead strings on the device
    Deltas only append to the two resident slabs.  gar_snapshot_compact rebuilds the slab of each selected group (`groups`: a
    mask of GAR_COMPACT_*) so that it holds exactly the strings the resident columns reference, entirely on the device: no byte
@@ -491,8 +529,8 @@ int gar_snapshot_apply_actual(gar_engine *e, const gar_actual_delta *d, gar_actu
      - strings are never shared afterwards: two references to the same bytes become two copies (only the key pair stays
        shared).  For a hand-packed table that interned strings slab_len may therefore grow; `out` reports it, it is no error.
      - row order, every CSR and every fixed-width column are untouched.  The slab keeps GAR_SLAB_PAD zero bytes behind slab_len.
-   Every later gar_diff, gar_diff_device, gar_diff_keys, gar_bindings_diff, gar_snapshot_apply_objects and
-   gar_snapshot_apply_actual answers bit for bit as before the call, except that tok_name / tok_region reference the new object
+   Every later gar_diff, gar_diff_device, gar_diff_keys, gar_bindings_diff, gar_snapshot_apply_objects,
+   gar_snapshot_apply_actual and gar_snapshot_apply_zones answers bit for bit as before the call, except that tok_name / tok_region reference the new object
    slab (equal as the strings they name; gar_snapshot_read_slab resolves them) and later deltas report slab_base / slab_len
    relative to the compacted slab.
    groups == 0 or unknown bits: GAR_E_INVALID.  GAR_E_STATE in exactly the cases of gar_snapshot_apply_objects.  The new slabs and
