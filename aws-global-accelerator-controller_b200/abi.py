@@ -173,6 +173,19 @@ class GarCompactResult(C.Structure):
     _fields_ = [(k, C.c_uint64) for k in ("obj_slab_before", "obj_slab_len", "act_slab_before", "act_slab_len")]
 
 
+class GarExportResult(C.Structure):
+    _fields_ = [(k, C.c_uint64) for k in ("obj_bytes", "act_bytes", "obj_slab_len", "act_slab_len")]
+
+
+class Exported:
+    """The resident tables exported to host memory (include/garecon.h gar_snapshot_export): .objects / .actual (GarObjects /
+    GarActual pointing into .buf; zeroed for a group not exported), .result (GarExportResult) and .buf, the uint8 array that
+    owns the bytes (the object group at offset 0, the AWS group at .act_at).  Engine.load(exported) restores it."""
+
+    def __init__(self, objects: GarObjects, actual: GarActual, result: GarExportResult, buf: np.ndarray, act_at: int):
+        self.objects, self.actual, self.result, self.buf, self.act_at = objects, actual, result, buf, act_at
+
+
 EGB_DELETING, EGB_HAS_FINALIZERS, EGB_OBSERVED = 1, 2, 4
 (OP_EGB_ADD_FINALIZER, OP_EGB_REMOVE_FINALIZER, OP_EGB_REMOVE_ENDPOINT, OP_EGB_ADD_ENDPOINT, OP_EGB_UPDATE_WEIGHT, OP_EGB_UPDATE_STATUS) = range(11, 17)
 ST_REQUEUE_1S = 8
@@ -329,6 +342,9 @@ def load_library(path: os.PathLike | None = None) -> C.CDLL:
     lib.gar_snapshot_apply_zones.restype = C.c_int
     lib.gar_snapshot_compact.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(GarCompactResult)]
     lib.gar_snapshot_compact.restype = C.c_int
+    lib.gar_snapshot_export.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.POINTER(GarObjects), C.c_void_p, C.c_uint64,
+                                        C.POINTER(GarActual), C.POINTER(GarExportResult)]
+    lib.gar_snapshot_export.restype = C.c_int
     lib.gar_snapshot_read_slab.argtypes = [C.c_void_p, C.c_uint32, C.c_uint64, C.c_uint64, C.c_void_p]
     lib.gar_snapshot_read_slab.restype = C.c_int
     lib.gar_shard_route.argtypes = [C.c_void_p, C.POINTER(GarShard), C.c_int, _u64p, _u64p]
@@ -364,7 +380,7 @@ def load_library(path: os.PathLike | None = None) -> C.CDLL:
 
 EXPORTED_SYMBOLS = (
     "gar_engine_create", "gar_engine_destroy", "gar_snapshot_load", "gar_snapshot_attach_device", "gar_diff",
-    "gar_diff_device", "gar_diff_keys", "gar_bindings_diff", "gar_snapshot_apply_objects", "gar_snapshot_apply_actual", "gar_snapshot_apply_zones", "gar_snapshot_compact", "gar_snapshot_read_slab", "gar_shard_route", "gar_shard_pack", "gar_shard_unpack", "gar_shard_blob_bytes",
+    "gar_diff_device", "gar_diff_keys", "gar_bindings_diff", "gar_snapshot_apply_objects", "gar_snapshot_apply_actual", "gar_snapshot_apply_zones", "gar_snapshot_compact", "gar_snapshot_export", "gar_snapshot_read_slab", "gar_shard_route", "gar_shard_pack", "gar_shard_unpack", "gar_shard_blob_bytes",
     "gar_shard_arena", "gar_shard_open_peers", "gar_shard_pack_peers",
     "gar_changeset_free", "gar_last_error", "gar_version", "gar_algorithmic_bytes",
     "gar_last_stage_timings", "gar_last_counters",
@@ -470,6 +486,31 @@ class Engine:
         res = GarCompactResult()
         self._check(self.lib.gar_snapshot_compact(self._h, int(groups), C.byref(res)))
         return res
+
+    def export_size(self, groups: int = COMPACT_OBJECTS | COMPACT_ACTUAL) -> GarExportResult:
+        """The size query of gar_snapshot_export: the buffer bytes and slab_len each selected group needs (runs the lengths pass
+        and the scan on the device)."""
+        res = GarExportResult()
+        self._check(self.lib.gar_snapshot_export(self._h, int(groups), None, 0, C.byref(GarObjects()), None, 0, C.byref(GarActual()), C.byref(res)))
+        return res
+
+    def export(self, groups: int = COMPACT_OBJECTS | COMPACT_ACTUAL, buf: np.ndarray | None = None) -> Exported:
+        """The resident tables of `groups` in the compacted layout, in host memory (include/garecon.h gar_snapshot_export): a size
+        query, then the export.  `buf`: a writable uint8 array to export into (e.g. a view of pinned memory), at least the
+        object group's bytes plus the AWS group's at the next 16-byte offset; None allocates one (pageable).  Nothing resident
+        changes."""
+        need = self.export_size(groups)
+        act_at = (int(need.obj_bytes) + 15) & ~15
+        total = act_at + int(need.act_bytes)
+        if buf is None:
+            buf = np.zeros(max(1, total), dtype=np.uint8)
+        if buf.dtype != np.uint8 or not buf.flags.c_contiguous or not buf.flags.writeable:
+            raise ValueError("buf must be a writable, contiguous uint8 array")
+        base = buf.ctypes.data
+        o, a, res = GarObjects(), GarActual(), GarExportResult()
+        self._check(self.lib.gar_snapshot_export(self._h, int(groups), C.c_void_p(base), min(int(need.obj_bytes), len(buf)), C.byref(o),
+                                                 C.c_void_p(base + act_at), max(0, min(int(need.act_bytes), len(buf) - act_at)), C.byref(a), C.byref(res)))
+        return Exported(o, a, res, buf, act_at)
 
     def read_slab(self, group: int, off: int, length: int) -> np.ndarray:
         """`length` bytes at `off` of the resident slab of `group` (COMPACT_OBJECTS or COMPACT_ACTUAL) as a uint8 array

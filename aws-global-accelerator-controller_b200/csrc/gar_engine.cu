@@ -527,11 +527,14 @@ __global__ void __launch_bounds__(256) k_shard_pack_rows(const __grid_constant__
 // bulk store (cp.async.bulk.global.shared::cta, as k_shard_pack_rows does).  Windows start at multiples of 16 bytes of a
 // 16-byte aligned slab, so only the last window has a tail that goes out by ordinary stores.  No warp loops over more than
 // COMPACT_LONG bytes of one string: longer strings are left out here and copied by k_compact_long, launched behind this kernel.
+// Block b copies window w0 + b into dst + b * COMPACT_WINDOW: w0 = 0 writes the whole new slab (the compaction), a later w0 one
+// chunk of it into a ring slot (the export).
 __global__ void __launch_bounds__(256) k_compact_copy(u8 *__restrict__ dst, const u8 *__restrict__ src, const gar_str *__restrict__ sref,
-                                                      const u64 *__restrict__ off, u32 m, u64 total) {
+                                                      const u64 *__restrict__ off, u32 m, u64 total, u32 w0) {
   __shared__ alignas(128) u8 tile[COMPACT_WINDOW];
   __shared__ u32 s_p[2];
-  const u64 lo = (u64)blockIdx.x * COMPACT_WINDOW, hi = min(lo + COMPACT_WINDOW, total);
+  const u64 lo = (u64)(w0 + blockIdx.x) * COMPACT_WINDOW, hi = min(lo + COMPACT_WINDOW, total);
+  dst += (u64)blockIdx.x * COMPACT_WINDOW;  // this window's first destination byte
   if (threadIdx.x == 0) s_p[0] = compact_first(off, m, lo);
   if (threadIdx.x == 32) s_p[1] = compact_end(off, m, hi);
   __syncthreads();
@@ -565,11 +568,11 @@ __global__ void __launch_bounds__(256) k_compact_copy(u8 *__restrict__ dst, cons
   __syncthreads();
   const u32 bytes = (u32)(hi - lo), body = bytes & ~15u;
   if (threadIdx.x == 0 && body) {
-    bulk_s2g(dst + lo, tile, body);
+    bulk_s2g(dst, tile, body);
     asm volatile("cp.async.bulk.commit_group;" ::: "memory");
     asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // the tile must stay until it has been read
   }
-  if (threadIdx.x >= 32 && threadIdx.x - 32 < bytes - body) dst[lo + body + threadIdx.x - 32] = tile[body + threadIdx.x - 32];
+  if (threadIdx.x >= 32 && threadIdx.x - 32 < bytes - body) dst[body + threadIdx.x - 32] = tile[body + threadIdx.x - 32];
 }
 // Strings longer than COMPACT_LONG, same windows: the block lists the long strings that overlap its window (at most
 // COMPACT_WINDOW / COMPACT_LONG + 2) and copies the part of each that falls inside with all 256 threads, 16 bytes per thread and
@@ -578,9 +581,10 @@ __global__ void __launch_bounds__(256) k_compact_copy(u8 *__restrict__ dst, cons
 // unaligned head and tail of the part go by bytes.
 constexpr u32 COMPACT_LONG_LIST = COMPACT_WINDOW / COMPACT_LONG + 2;
 __global__ void __launch_bounds__(256) k_compact_long(u8 *__restrict__ dst, const u8 *__restrict__ src, const gar_str *__restrict__ sref,
-                                                      const u64 *__restrict__ off, u32 m, u64 total) {
+                                                      const u64 *__restrict__ off, u32 m, u64 total, u32 w0) {
   __shared__ u32 s_p[2], s_n, s_list[COMPACT_LONG_LIST];
-  const u64 lo = (u64)blockIdx.x * COMPACT_WINDOW, hi = min(lo + COMPACT_WINDOW, total);
+  const u64 lo = (u64)(w0 + blockIdx.x) * COMPACT_WINDOW, hi = min(lo + COMPACT_WINDOW, total);
+  dst += (u64)blockIdx.x * COMPACT_WINDOW - lo;  // destination byte k of the slab goes to dst[k]
   if (threadIdx.x == 0) {
     s_p[0] = compact_first(off, m, lo);
     s_n = 0;
@@ -760,6 +764,18 @@ struct gar_engine {
     }
     return b.p;
   }
+  // a buffer no recorded launch sequence holds (staging of deltas, compaction and export): it grows without dropping the graph
+  void *own_ensure(DBuf &b, size_t bytes) {
+    bytes = (bytes + 255) & ~(size_t)255;
+    if (b.cap < bytes) {
+      if (b.p) CK(cudaFree(b.p));
+      b = DBuf{};
+      size_t want = bytes + bytes / 4;
+      CK(cudaMalloc(&b.p, want));
+      b.cap = want;
+    }
+    return b.p;
+  }
   void *pin_ensure(DBuf &b, size_t bytes) {
     if (bytes < 64) bytes = 64;
     if (b.cap < bytes) {
@@ -912,15 +928,18 @@ struct gar_engine {
   void copy32(u32 *dst, const u32 *src, size_t n) {
     if (n) CK(cudaMemcpyAsync(dst, src, n * 4, cudaMemcpyDeviceToDevice, stream));
   }
-  void exclusive_scan(u32 *data, u32 n) { scan(data, n); }
-  void exclusive_scan(u64 *data, u32 n) { scan(data, n); }
+  void exclusive_scan(u32 *data, u32 n) { scan(data, n, (unsigned long long *)nullptr); }
+  // the 64-bit scan is the compaction's and the export's: its tile states are its own, so an export grows no buffer that a
+  // recorded launch sequence holds
+  DBuf compact_tiles;
+  void exclusive_scan(u64 *data, u32 n) { scan(data, n, (unsigned long long *)own_ensure(compact_tiles, 8 * (size_t)((n + SCAN_TILE - 1) / SCAN_TILE + 2))); }
   template <class V>
-  void scan(V *data, u32 n) {
+  void scan(V *data, u32 n, unsigned long long *state) {
     if (!n) return;
     stage_begin("exclusive_scan");
     u32 ntiles = (n + SCAN_TILE - 1) / SCAN_TILE;
     size_t sbytes = 8 * (size_t)(ntiles + 2);
-    unsigned long long *state = (unsigned long long *)dev_ensure(d_scan_tiles, sbytes);
+    if (!state) state = (unsigned long long *)dev_ensure(d_scan_tiles, sbytes);
     CK(cudaMemsetAsync(state, 0, sbytes, stream));  // tile states + the ticket counter (last word)
     k_scan_lookback<V><<<ntiles, SCAN_THREADS, 0, stream>>>(data, n, state, (u32 *)(state + ntiles + 1));
     launches += 1;
@@ -983,7 +1002,7 @@ struct gar_engine {
   void upload(void *dst, const void *src, size_t bytes) {
     if (bytes) CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, stream));
   }
-  void *delta_scratch(int k, size_t bytes) { return dev_ensure(dscratch[k], bytes); }
+  void *delta_scratch(int k, size_t bytes) { return own_ensure(dscratch[k], bytes); }
   void *delta_col(int c, size_t bytes) { return dev_ensure(o_set == 0 ? dset[c] : in[c], bytes); }
   void delta_swap() { o_set ^= 1; }
   u8 *delta_slab(u64 keep, u64 need) { return grow_slab(in[DC_N], keep, need); }
@@ -1031,17 +1050,93 @@ struct gar_engine {
     CK(cudaFree(b.p));
     b = DBuf{};
   }
-  void compact_copy(u8 *dst, const u8 *src, const gar_str *sref, const u64 *off, u32 m, u64 total, bool any_long) {
-    if (!total) return;
+  // windows [w0, w1) of the new slab into dst (dst[0] = destination byte w0 * COMPACT_WINDOW); by default all of them
+  void compact_copy(u8 *dst, const u8 *src, const gar_str *sref, const u64 *off, u32 m, u64 total, bool any_long, u32 w0 = 0, u32 w1 = ~0u) {
     const u32 windows = (u32)((total + COMPACT_WINDOW - 1) / COMPACT_WINDOW);
+    if (w1 > windows) w1 = windows;
+    if (w0 >= w1) return;
     stage_begin("compact_copy");
-    k_compact_copy<<<windows, 256, 0, stream>>>(dst, src, sref, off, m, total);
+    k_compact_copy<<<w1 - w0, 256, 0, stream>>>(dst, src, sref, off, m, total, w0);
     launches++;
     if (any_long) {
-      k_compact_long<<<windows, 256, 0, stream>>>(dst, src, sref, off, m, total);
+      k_compact_long<<<w1 - w0, 256, 0, stream>>>(dst, src, sref, off, m, total, w0);
       launches++;
     }
     stage_end();
+  }
+
+  // ---- export (gar_compact.h, gar_snapshot_export).  The new slab is gathered EXPORT_CHUNK windows at a time into a ring of
+  // EXPORT_RING device slots; a copy stream takes each chunk to the caller's buffer as soon as it is gathered, and a slot is
+  // gathered into again only after its previous copy has completed.  Device memory: the ring, not a second slab.
+  cudaStream_t xstream = nullptr;
+  cudaEvent_t x_fence = nullptr, x_gathered[EXPORT_RING] = {}, x_copied[EXPORT_RING] = {};
+  DBuf x_stage[CG_N], x_ring;
+  void *try_alloc(DBuf &b, size_t bytes) {
+    if (b.cap < bytes) {
+      CK(cudaFree(b.p));
+      b = DBuf{};
+      if (cudaMalloc(&b.p, bytes) != cudaSuccess) {
+        cudaGetLastError();
+        b.p = nullptr;
+        return nullptr;
+      }
+      b.cap = bytes;
+    }
+    return b.p;
+  }
+  void *export_stage(int g, size_t bytes) { return try_alloc(x_stage[g], bytes); }
+  void *export_scratch(int k, size_t bytes) { return try_alloc(dscratch[k], bytes); }
+  void export_fence() {
+    if (!xstream) {
+      CK(cudaStreamCreateWithFlags(&xstream, cudaStreamNonBlocking));
+      CK(cudaEventCreateWithFlags(&x_fence, cudaEventDisableTiming));
+      for (int s = 0; s < EXPORT_RING; s++) {
+        CK(cudaEventCreateWithFlags(&x_gathered[s], cudaEventDisableTiming));
+        CK(cudaEventCreateWithFlags(&x_copied[s], cudaEventDisableTiming));
+      }
+    }
+    CK(cudaEventRecord(x_fence, stream));
+    CK(cudaStreamWaitEvent(xstream, x_fence, 0));
+  }
+  void export_copy(void *host, const void *dev, size_t bytes) {
+    if (bytes) CK(cudaMemcpyAsync(host, dev, bytes, cudaMemcpyDeviceToHost, xstream));
+  }
+  int export_slab(u8 *host, const u8 *src, const gar_str *sref, const u64 *off, u32 m, u64 total, bool any_long) {
+    const u32 windows = (u32)((total + COMPACT_WINDOW - 1) / COMPACT_WINDOW);
+    if (!windows) return GAR_OK;
+    const size_t slot_bytes = (size_t)EXPORT_CHUNK * COMPACT_WINDOW;
+    u8 *ring = (u8 *)try_alloc(x_ring, EXPORT_RING * slot_bytes);
+    if (!ring) return GAR_E_NOMEM;
+    stage_begin("export_slab");
+    for (u32 w0 = 0, k = 0; w0 < windows; w0 += EXPORT_CHUNK, k++) {
+      const int s = (int)(k % EXPORT_RING);
+      u8 *slot = ring + s * slot_bytes;
+      // the slot's previous chunk has left, also one of an earlier group of this call (k starts at 0 per group).  Before the
+      // slot's first use in a call the event was never recorded or has completed (export_end drains the copy stream): no wait
+      CK(cudaStreamWaitEvent(stream, x_copied[s], 0));
+      compact_copy(slot, src, sref, off, m, total, any_long, w0, w0 + EXPORT_CHUNK);
+      CK(cudaEventRecord(x_gathered[s], stream));
+      CK(cudaStreamWaitEvent(xstream, x_gathered[s], 0));
+      const u64 lo = (u64)w0 * COMPACT_WINDOW, hi = std::min<u64>(lo + slot_bytes, total);
+      CK(cudaMemcpyAsync(host + lo, slot, hi - lo, cudaMemcpyDeviceToHost, xstream));
+      CK(cudaEventRecord(x_copied[s], xstream));
+    }
+    stage_end();
+    return GAR_OK;
+  }
+  // both streams drained (the caller's buffer is not written after the call returns), the per-string staging and the export's
+  // buffers freed: they are as large as the reference columns
+  void export_end() {
+    const cudaError_t a = cudaStreamSynchronize(stream), b = xstream ? cudaStreamSynchronize(xstream) : cudaSuccess;
+    for (int g = 0; g < CG_N; g++)
+      for (DBuf *d : {&dscratch[CS_SREF + g], &dscratch[CS_OFF + g], &x_stage[g]}) {
+        cudaFree(d->p);
+        *d = DBuf{};
+      }
+    cudaFree(x_ring.p);
+    x_ring = DBuf{};
+    CK(a);
+    CK(b);
   }
 };
 
@@ -1357,6 +1452,36 @@ static void do_compact(gar_engine *e, u32 groups, gar_compact_result *out) {
   }
 }
 
+static void do_export(gar_engine *e, u32 groups, void *obj_buf, u64 obj_cap, gar_objects *obj_out, void *act_buf, u64 act_cap, gar_actual *act_out,
+                      gar_export_result *out) {
+  if (!groups || (groups & ~(u32)(GAR_COMPACT_OBJECTS | GAR_COMPACT_ACTUAL))) throw InvalidError{"groups must be a non-empty mask of GAR_COMPACT_OBJECTS | GAR_COMPACT_ACTUAL"};
+  if (((groups & GAR_COMPACT_OBJECTS) && !obj_out) || ((groups & GAR_COMPACT_ACTUAL) && !act_out)) throw InvalidError{"NULL table struct for a selected group"};
+  if (!e->loaded) throw StateError{"no snapshot loaded"};
+  if (e->shard_home || e->shard_round != 0) throw StateError{"export is not available in sharded mode"};
+  CK(cudaSetDevice(e->device));
+  e->marks.clear();
+  e->events_used = 0;
+  e->stage_depth = 0;
+  // reads only: the resident tables, the prepared state and the recorded launch sequence stay as they are
+  u8 *const buf[CG_N] = {(groups & GAR_COMPACT_OBJECTS) ? (u8 *)obj_buf : nullptr, (groups & GAR_COMPACT_ACTUAL) ? (u8 *)act_buf : nullptr};
+  const u64 cap[CG_N] = {obj_cap, act_cap};
+  Compactor<gar_engine> C{*e, e->T};
+  int rc;
+  try {
+    rc = C.export_to(groups, buf, cap, obj_out, act_out, *out);
+  } catch (const CudaError &) {
+    try {
+      e->export_end();
+    } catch (const CudaError &) {
+    }
+    throw;
+  }
+  e->export_end();
+  CK(cudaGetLastError());
+  if (rc == GAR_E_NOMEM) throw DeviceMemoryError{C.error};
+  if (rc != GAR_OK) throw InvalidError{C.error};
+}
+
 static void do_read_slab(gar_engine *e, u32 group, u64 off, u64 len, void *dst) {
   if (group != GAR_COMPACT_OBJECTS && group != GAR_COMPACT_ACTUAL) throw InvalidError{"group must be GAR_COMPACT_OBJECTS or GAR_COMPACT_ACTUAL"};
   if (!e->loaded) throw StateError{"no snapshot loaded"};
@@ -1655,6 +1780,12 @@ void gar_engine_destroy(gar_engine *e) {
   for (auto &b : e->dscratch) cudaFree(b.p);
   for (auto &b : e->aset) cudaFree(b.p);
   for (auto &b : e->compact_new) cudaFree(b.p);
+  for (auto &b : e->x_stage) cudaFree(b.p);
+  for (DBuf *b : {&e->x_ring, &e->compact_tiles}) cudaFree(b->p);
+  if (e->xstream) cudaStreamDestroy(e->xstream);
+  for (cudaEvent_t ev : {e->x_fence}) if (ev) cudaEventDestroy(ev);
+  for (int s = 0; s < EXPORT_RING; s++)
+    for (cudaEvent_t ev : {e->x_gathered[s], e->x_copied[s]}) if (ev) cudaEventDestroy(ev);
   cudaFree(e->d_valid.p);
   for (int k = 0; k < 2; k++) {
     if (e->dl_pin[k].p) cudaFreeHost(e->dl_pin[k].p);
@@ -1740,6 +1871,12 @@ int gar_snapshot_apply_zones(gar_engine *e, const gar_zone_delta *d, gar_zone_de
 int gar_snapshot_compact(gar_engine *e, uint32_t groups, gar_compact_result *out) {
   if (!out) return GAR_E_INVALID;
   return guarded(e, [&] { do_compact(e, groups, out); });
+}
+
+int gar_snapshot_export(gar_engine *e, uint32_t groups, void *obj_buf, uint64_t obj_cap, gar_objects *obj_out, void *act_buf, uint64_t act_cap,
+                        gar_actual *act_out, gar_export_result *out) {
+  if (!out) return GAR_E_INVALID;
+  return guarded(e, [&] { do_export(e, groups, obj_buf, obj_cap, obj_out, act_buf, act_cap, act_out, out); });
 }
 
 int gar_snapshot_read_slab(gar_engine *e, uint32_t group, uint64_t off, uint64_t len, void *dst) {

@@ -547,6 +547,35 @@ typedef struct gar_compact_result {
 } gar_compact_result;
 int gar_snapshot_compact(gar_engine *e, uint32_t groups, gar_compact_result *out);
 
+/* ---------------------------------------------------------------- export: the resident tables in host memory
+   gar_snapshot_export copies the tables of each selected group (`groups`: a mask of GAR_COMPACT_*) into a host buffer of the
+   caller, so that a snapshot kept current by deltas (the only up-to-date copy of the AWS side) can be checkpointed and later
+   restored with one gar_snapshot_load instead of a re-list.
+     - what is exported: the tables gar_snapshot_compact(groups) would leave resident at this moment: the same row order, CSRs
+       and fixed-width columns, and the compaction layout above for the gar_str columns and the slab (the object key copied
+       once, obj_ingress_class without its flag and rec_alias_dns without an alias empty, interned strings un-shared).  Right
+       after a compaction the exported slab equals the resident one byte for byte.
+     - buffer layout: the columns of the group in struct declaration order, each at a 16-byte aligned offset from the start of
+       the buffer, the slab (slab_len bytes) last.  *obj_out / *act_out get the counts, slab_len and pointers into the buffer, so
+       gar_snapshot_load(e2, obj_out, act_out) restores them directly; one exported group may be paired with a freshly packed
+       table of the other (AWS tables from a checkpoint with a fresh informer list).
+     - size query: obj_buf / act_buf == NULL for a selected group fills out->*_bytes / *_slab_len and writes nothing for that
+       group.  The query runs the lengths pass and the scan of the export, so it costs device work.  A cap below the bytes
+       needed returns GAR_E_INVALID with the needed bytes in `out`; nothing is written past the cap.
+     - nothing resident changes: slabs, columns, the prepared state (digests, indexes, owned lists) and the recorded launch
+       sequence stay as they were; the next diff replays if it would have replayed before.  The call only reads, so an attached
+       snapshot can be exported too.
+     - pinned host memory lets the copy overlap the gather on the device; pageable memory gives the same bytes, more slowly.
+   GAR_E_INVALID: groups == 0 or unknown bits, a NULL *_out for a selected group, a buffer too small.  GAR_E_STATE before a load,
+   on a sharded sub-snapshot and once gar_shard_route has run on the loaded slice.  GAR_E_NOMEM: device staging could not be
+   allocated; the snapshot is unchanged.  A CUDA error returns GAR_E_CUDA and leaves the snapshot loaded, as a diff does. */
+typedef struct gar_export_result {
+  uint64_t obj_bytes, act_bytes;        /* buffer bytes the selected groups need (and, on success, used); 0 for a group not selected */
+  uint64_t obj_slab_len, act_slab_len;  /* slab_len of the exported tables */
+} gar_export_result;
+int gar_snapshot_export(gar_engine *e, uint32_t groups, void *obj_buf, uint64_t obj_cap, gar_objects *obj_out, void *act_buf, uint64_t act_cap,
+                        gar_actual *act_out, gar_export_result *out);
+
 /* Copies `len` bytes at `off` of a resident slab to host memory (group = GAR_COMPACT_OBJECTS or GAR_COMPACT_ACTUAL, exactly one):
    how a caller reads the strings tok_name / tok_region name without mirroring the slab itself.  off + len beyond the resident
    slab_len, or a group that is not exactly one of the two: GAR_E_INVALID.  GAR_E_STATE before a load and on a sharded
