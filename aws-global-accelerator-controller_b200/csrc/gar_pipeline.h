@@ -553,15 +553,12 @@ struct FGatherHeader {
   u32 *flags;
   GAR_HD void operator()(u32) const { flags[FW_NDPORTS] = *ndports; }
 };
-// the two per-value joins in one pass (independent probe chains overlap): first alias record under the value's (zone, name),
-// and the object the value names (which also says whether it is an orphan)
+// the two per-value joins in one pass (their probe chains overlap: value_joins): first alias record under the value's
+// (zone, name), and the object the value names (which also says whether it is an orphan)
 struct FValueJoins {
   DevTables T;
   Work W;
-  GAR_HD void operator()(u32 v) const {
-    link_value_alias(T, W, v);
-    resolve_value(T, W, v);
-  }
+  GAR_HD void operator()(u32 v) const { value_joins(T, W, v); }
 };
 // the object half of FValueJoins, alone: re-run after an object delta (the alias links read the actual side only)
 struct FResolveValue {

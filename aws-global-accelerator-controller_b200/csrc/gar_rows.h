@@ -1213,19 +1213,6 @@ GAR_HD OwnedHit owned_get(const DevTables &T, const Work &W, const Owned &o, u32
   return h;
 }
 
-// first alias record with type A under (zone, name): row and its alias DNSName ref  (rows of a bucket are ascending)
-GAR_HD u32 first_alias_a(const DevTables &T, const Work &W, u32 zone, Str name, u64 name_hash, gar_str *alias_dns) {
-  Cursor c = idx_open(W.ix_alias, key_hash_zoned_h(zone, name_hash));
-  IdxEntry e;
-  while (idx_next(W.ix_alias, c, &e)) {
-    if (e.a0 != zone || e.a1 != GAR_RR_A) continue;
-    if (streq(mkstr(T.a.slab, e.s0), name)) {
-      *alias_dns = e.s1;
-      return e.row;
-    }
-  }
-  return GAR_NONE;
-}
 // smallest alias record row > after under (zone, name), any type
 GAR_HD u32 next_alias_any(const DevTables &T, const Work &W, u32 zone, Str name, u32 after /* GAR_NONE = none yet */) {
   Cursor c = idx_open(W.ix_alias, key_hash_zoned(zone, name));
@@ -1423,26 +1410,12 @@ GAR_HD u32 r53_reconcile(const DevTables &T, const Work &W, u32 i, bool valid, O
 // ------------------------------------------------------------------ (a9) Route53 ensure, relational form
 //
 // The same decisions as r53_reconcile for the common shape (one lbIngress), split into uniform data-parallel steps:
-//   link_value_alias  per owner value row : first alias A record under the same (zone, name)       [build side, once]
+//   value_joins       per owner value row : first alias A record under the same (zone, name)       [build side, once]
 //   r53_prepare       per object          : filter, accelerator by target hostname, number of hostnames
 //   r53_fill_pairs    per object          : (object, k, hostname slice) rows
 //   r53_pair          per (object, k)     : GetHostedZone + findARecord over the object's owned names + needRecordsUpdate
 //   r53_combine       per object          : replay the pair results in order (first NO_ZONE ends the stream), emit ops
 // Objects of any other shape go through r53_reconcile inside r53_combine.
-
-GAR_HD void link_value_alias(const DevTables &T, const Work &W, u32 v) {
-  u32 row = GAR_NONE;
-  gar_str dns = 0;
-  if (W.val_cls[v] != VAL_NOT_OWNER) {
-    u32 rec = W.val_rec[v];
-    row = first_alias_a(T, W, W.rec_zone[rec], mkstr(T.a.slab, T.a.rec_name[rec]), W.rec_name_hash[rec], &dns);
-  }
-  ValLink l;
-  l.alias_row = row;
-  l.pad = 0;
-  l.alias_dns = dns;
-  W.val_link[v] = l;
-}
 
 // warp-synchronous.  Writes r53_mode, r53_acc, r53_acc_dns, pair count (into pair_begin[i]) and, for objects that
 // are finished here, the status word.
@@ -1666,6 +1639,60 @@ GAR_HD void resolve_value(const DevTables &T, const Work &W, u32 v) {
   const u8 orphan = (cls & VAL_OWNER_3PART) && o == GAR_NONE ? 1 : 0;
   if (orphan) {
     u32 rec = W.val_rec[v];
+    ix_count(W.hist[IX_OVN], key_hash_zoned_h(W.rec_zone[rec], W.rec_name_hash[rec]));
+  }
+  W.val_orphan[v] = orphan;
+}
+
+// Both joins of one value in the full prepare: the first alias A record under the value's (zone, name) (ValLink) and what
+// resolve_value answers.  Every
+// row-local read, both buckets' bounds and both buckets' first entries are issued before either bucket is walked, so the two
+// probe chains overlap instead of running one after the other (each walk still takes the first entry whose tag, fields and
+// full key bytes match).
+GAR_HD void value_joins(const DevTables &T, const Work &W, u32 v) {
+  const u32 cls = W.val_cls[v];
+  u32 row = GAR_NONE, o = GAR_NONE;
+  gar_str dns = 0;
+  if (cls != VAL_NOT_OWNER) {
+    const u32 rec = W.val_rec[v], kind = (cls & VAL_OWNER_INGRESS) ? 1u : 0u;
+    const gar_str kref = W.val_key[v];
+    const u64 kh = W.val_key_hash[v];
+    const u32 zone = W.rec_zone[rec];
+    const gar_str nref = T.a.rec_name[rec];
+    const u64 nh = W.rec_name_hash[rec];
+    Cursor ca = idx_open(W.ix_alias, key_hash_zoned_h(zone, nh)), co = idx_open(W.ix_obj, kh);
+    IdxEntry ea, eo;
+    ea.tag = ~ca.tag;
+    eo.tag = ~co.tag;
+    if (ca.pos < ca.end) ea = load_entry(W.ix_alias.ent + ca.pos);
+    if (co.pos < co.end) eo = load_entry(W.ix_obj.ent + co.pos);
+    const Str name = mkstr(T.a.slab, nref), key = mkstr(T.a.slab, kref);
+    while (ca.pos < ca.end) {  // the first alias record of type A (rows of a bucket are ascending)
+      if (ea.tag == ca.tag && ea.a0 == zone && ea.a1 == GAR_RR_A && streq(mkstr(T.a.slab, ea.s0), name)) {
+        row = ea.row;
+        dns = ea.s1;
+        break;
+      }
+      if (++ca.pos < ca.end) ea = load_entry(W.ix_alias.ent + ca.pos);
+    }
+    while (co.pos < co.end) {  // find_object: the canonical row
+      if (eo.tag == co.tag && eo.a0 == kind && streq(mkstr(T.o.slab, eo.s0), key)) {
+        o = eo.row;
+        break;
+      }
+      if (++co.pos < co.end) eo = load_entry(W.ix_obj.ent + co.pos);
+    }
+    if (o != GAR_NONE) GAR_HIST_ADD(&W.own_begin[2 * o + 1]);
+  }
+  ValLink l;
+  l.alias_row = row;
+  l.pad = 0;
+  l.alias_dns = dns;
+  W.val_link[v] = l;
+  W.val_obj[v] = o;
+  const u8 orphan = (cls & VAL_OWNER_3PART) && o == GAR_NONE ? 1 : 0;
+  if (orphan) {
+    const u32 rec = W.val_rec[v];
     ix_count(W.hist[IX_OVN], key_hash_zoned_h(W.rec_zone[rec], W.rec_name_hash[rec]));
   }
   W.val_orphan[v] = orphan;
