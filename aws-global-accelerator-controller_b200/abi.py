@@ -99,6 +99,25 @@ class GarKeyset(C.Structure):
     _fields_ = [("n_rows", C.c_uint32), ("rows", _u32p), ("n_deleted", C.c_uint32), ("deleted_kind", _u8p), ("deleted_key", C.POINTER(C.c_char_p))]
 
 
+class GarReadSet(C.Structure):
+    _fields_ = [("n_lbs", C.c_uint32), ("lb_rows", _u32p), ("n_lb_misses", C.c_uint32), ("lb_miss_obj", _u32p), ("lb_miss_j", _u32p),
+                ("lb_miss_name", _u64p), ("lb_miss_region", _u64p), ("n_accels", C.c_uint32), ("acc_rows", _u32p), ("n_zones", C.c_uint32),
+                ("zone_rows", _u32p), ("opaque", C.c_void_p)]
+
+
+class ReadSet:
+    """gar_read_set's result as numpy arrays: lb_rows, acc_rows, zone_rows (ascending, distinct resident rows) and the LB misses
+    (lb_miss_obj, lb_miss_j, and lb_miss_name / lb_miss_region as gar_str refs into the resident object slab)."""
+
+    FIELDS = ("lb_rows", "acc_rows", "zone_rows", "lb_miss_obj", "lb_miss_j", "lb_miss_name", "lb_miss_region")
+
+    def __init__(self, rs: GarReadSet):
+        n = {"lb_rows": rs.n_lbs, "acc_rows": rs.n_accels, "zone_rows": rs.n_zones}
+        for k in self.FIELDS:
+            cnt = n.get(k, rs.n_lb_misses)
+            setattr(self, k, _np_from(getattr(rs, k), cnt, np.uint64 if k in ("lb_miss_name", "lb_miss_region") else np.uint32))
+
+
 class GarBindings(C.Structure):
     _fields_ = [
         ("n_bindings", C.c_uint32), ("egb_flags", _u8p), ("egb_ref_kind", _u8p), ("egb_ref_key", _u64p), ("egb_eg_arn", _u64p),
@@ -332,6 +351,10 @@ def load_library(path: os.PathLike | None = None) -> C.CDLL:
         getattr(lib, fn).restype = C.c_int
     lib.gar_diff_keys.argtypes = [C.c_void_p, C.POINTER(GarKeyset), C.POINTER(GarChangeset)]
     lib.gar_diff_keys.restype = C.c_int
+    lib.gar_read_set.argtypes = [C.c_void_p, C.POINTER(GarKeyset), C.POINTER(GarReadSet)]
+    lib.gar_read_set.restype = C.c_int
+    lib.gar_read_set_free.argtypes = [C.c_void_p, C.POINTER(GarReadSet)]
+    lib.gar_read_set_free.restype = None
     lib.gar_bindings_diff.argtypes = [C.c_void_p, C.POINTER(GarBindings), C.POINTER(GarChangeset)]
     lib.gar_bindings_diff.restype = C.c_int
     lib.gar_snapshot_apply_objects.argtypes = [C.c_void_p, C.POINTER(GarObjectDelta), C.POINTER(GarDeltaResult)]
@@ -380,7 +403,7 @@ def load_library(path: os.PathLike | None = None) -> C.CDLL:
 
 EXPORTED_SYMBOLS = (
     "gar_engine_create", "gar_engine_destroy", "gar_snapshot_load", "gar_snapshot_attach_device", "gar_diff",
-    "gar_diff_device", "gar_diff_keys", "gar_bindings_diff", "gar_snapshot_apply_objects", "gar_snapshot_apply_actual", "gar_snapshot_apply_zones", "gar_snapshot_compact", "gar_snapshot_export", "gar_snapshot_read_slab", "gar_shard_route", "gar_shard_pack", "gar_shard_unpack", "gar_shard_blob_bytes",
+    "gar_diff_device", "gar_diff_keys", "gar_read_set", "gar_read_set_free", "gar_bindings_diff", "gar_snapshot_apply_objects", "gar_snapshot_apply_actual", "gar_snapshot_apply_zones", "gar_snapshot_compact", "gar_snapshot_export", "gar_snapshot_read_slab", "gar_shard_route", "gar_shard_pack", "gar_shard_unpack", "gar_shard_blob_bytes",
     "gar_shard_arena", "gar_shard_open_peers", "gar_shard_pack_peers",
     "gar_changeset_free", "gar_last_error", "gar_version", "gar_algorithmic_bytes",
     "gar_last_stage_timings", "gar_last_counters",
@@ -440,6 +463,18 @@ class Engine:
             out = ChangeSet(cs, keyset=True)
         finally:
             self.lib.gar_changeset_free(self._h, C.byref(cs))
+        return out
+
+    def read_set(self, rows, deleted=()) -> ReadSet:
+        """The resident AWS rows the decisions of this keyset read (include/garecon.h gar_read_set): what a worker re-describes
+        and applies with apply_actual before diff_keys(rows, deleted)."""
+        ks = make_keyset(rows, deleted)
+        rs = GarReadSet()
+        self._check(self.lib.gar_read_set(self._h, C.byref(ks), C.byref(rs)))
+        try:
+            out = ReadSet(rs)
+        finally:
+            self.lib.gar_read_set_free(self._h, C.byref(rs))
         return out
 
     def apply_objects(self, upserts: GarObjects | None = None, deleted=()) -> DeltaResult:

@@ -447,6 +447,9 @@ struct DBuf {
 struct HostResult {  // pinned host buffers of one change set
   DBuf status_ga, status_r53, derived, ops, tok_code, tok_name, tok_region, dport_begin, dports, obj_gid;
 };
+struct HostReadSet {  // pinned host buffers of one read set
+  DBuf rows, strs;
+};
 
 #define CK(call)                                                                                             \
   do {                                                                                                       \
@@ -709,6 +712,11 @@ struct gar_engine {
       }
   }
   std::vector<HostResult *> free_results;
+  std::vector<HostReadSet *> free_read_sets;
+  // read set (gar_read_set): scratch no recorded launch sequence holds, and what its bitmaps are known to hold
+  DBuf rs_buf[8];
+  ReadSetClean rs_clean;
+  void *read_set_buf(int k, size_t bytes) { return own_ensure(rs_buf[k], bytes); }
   float ms_h2d = 0;
   u32 launches = 0;
   u64 input_bytes = 0;  // slabs + fixed-width columns, each once
@@ -1494,6 +1502,98 @@ static void do_read_slab(gar_engine *e, u32 group, u64 off, u64 len, void *dst) 
   if (len) e->download(dst, slab + off, len);
 }
 
+// a key batch (gar_diff_keys, gar_read_set): checked, then copied to the device
+static void check_keyset(const gar_engine *e, const gar_keyset *ks) {
+  if ((ks->n_rows && !ks->rows) || (ks->n_deleted && (!ks->deleted_kind || !ks->deleted_key))) throw InvalidError{"NULL key set arrays"};
+  for (u32 k = 0; k < ks->n_rows; k++)
+    if (ks->rows[k] >= e->T.o.n_objects) throw InvalidError{"key set row out of range"};
+  for (u32 k = 0; k < ks->n_deleted; k++)
+    if (!ks->deleted_key[k] || ks->deleted_kind[k] > GAR_KIND_INGRESS) throw InvalidError{"bad deleted key"};
+}
+static void upload_keyset(gar_engine *e, const gar_keyset *ks, const u32 **rows_out, DelKeys *D) {
+  check_keyset(e, ks);
+  u32 *rows = (u32 *)e->dev_ensure(e->d_key_rows, 4 * (size_t)(ks->n_rows + 1));
+  if (ks->n_rows) CK(cudaMemcpyAsync(rows, ks->rows, 4 * (size_t)ks->n_rows, cudaMemcpyHostToDevice, e->stream));
+  std::vector<u8> slab;
+  std::vector<gar_str> refs(ks->n_deleted);
+  std::vector<u8> kinds(ks->n_deleted);
+  for (u32 k = 0; k < ks->n_deleted; k++) {
+    size_t len = strlen(ks->deleted_key[k]);
+    refs[k] = GAR_STR(slab.size(), len);
+    slab.insert(slab.end(), ks->deleted_key[k], ks->deleted_key[k] + len);
+    kinds[k] = ks->deleted_kind[k];
+  }
+  slab.resize(slab.size() + GAR_SLAB_PAD, 0);
+  u8 *dslab = (u8 *)e->dev_ensure(e->d_del_slab, slab.size());
+  u8 *dkind = (u8 *)e->dev_ensure(e->d_del_kind, ks->n_deleted + 1);
+  gar_str *dkey = (gar_str *)e->dev_ensure(e->d_del_key, 8 * (size_t)(ks->n_deleted + 1));
+  CK(cudaMemcpyAsync(dslab, slab.data(), slab.size(), cudaMemcpyHostToDevice, e->stream));
+  if (ks->n_deleted) {
+    CK(cudaMemcpyAsync(dkind, kinds.data(), ks->n_deleted, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(dkey, refs.data(), 8 * (size_t)ks->n_deleted, cudaMemcpyHostToDevice, e->stream));
+  }
+  CK(cudaStreamSynchronize(e->stream));  // the staging vectors go out of scope
+  *rows_out = rows;
+  *D = DelKeys{dkind, dkey, dslab};
+}
+
+static void do_read_set(gar_engine *e, const gar_keyset *ks, gar_readset *out) {
+  memset(out, 0, sizeof(*out));
+  if (!e->loaded) throw StateError{"no snapshot loaded"};
+  if (e->shard_home || e->shard_round != 0) throw StateError{"the read set is not available in sharded mode"};
+  check_keyset(e, ks);
+  CK(cudaSetDevice(e->device));
+  e->launches = 0;
+  e->marks.clear();
+  e->events_used = 0;
+  e->stage_depth = 0;
+  const u32 *rows;
+  DelKeys D;
+  upload_keyset(e, ks, &rows, &D);
+  Pipeline<gar_engine> &P = ensure_pipe(e);
+  P.orphan_sweep = !e->no_orphans;
+  P.allow_empty_cache = e->allow_empty_cache;
+  if (e->reprepare) P.prepared = false;
+  ReadSetter<gar_engine, Pipeline<gar_engine>> R{*e, P, e->rs_clean};
+  const int rc = R.run(rows, ks->n_rows, D, ks->n_deleted);
+  if (rc == GAR_E_INVALID) throw InvalidError{"objects layout rule violated: obj_ns and obj_name must be slices of one \"ns/name\" key string"};
+  if (rc != GAR_OK) throw InvalidError{"the snapshot did not settle: an intermediate relation kept outgrowing its buffer"};
+  HostReadSet *h;
+  if (!e->free_read_sets.empty()) {
+    h = e->free_read_sets.back();
+    e->free_read_sets.pop_back();
+  } else {
+    h = new HostReadSet();
+  }
+  out->opaque = h;
+  const u32 nl = R.n[RS_LB], na = R.n[RS_ACC], nz = R.n[RS_ZONE], nm = R.n[RS_MISS];
+  u32 *hr = (u32 *)e->pin_ensure(h->rows, 4 * ((size_t)nl + na + nz + 2 * (size_t)nm));
+  gar_str *hs = (gar_str *)e->pin_ensure(h->strs, 8 * 2 * (size_t)nm);
+  auto pull = [&](void *dst, const void *src, size_t bytes) {
+    if (bytes) CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, e->stream));
+  };
+  pull(hr, R.out.rows[RS_LB], 4 * (size_t)nl);
+  pull(hr + nl, R.out.rows[RS_ACC], 4 * (size_t)na);
+  pull(hr + nl + na, R.out.rows[RS_ZONE], 4 * (size_t)nz);
+  pull(hr + nl + na + nz, R.out.miss_obj, 4 * (size_t)nm);
+  pull(hr + nl + na + nz + nm, R.out.miss_j, 4 * (size_t)nm);
+  pull(hs, R.out.miss_name, 8 * (size_t)nm);
+  pull(hs + nm, R.out.miss_region, 8 * (size_t)nm);
+  CK(cudaStreamSynchronize(e->stream));
+  CK(cudaGetLastError());
+  out->n_lbs = nl;
+  out->lb_rows = hr;
+  out->n_accels = na;
+  out->acc_rows = hr + nl;
+  out->n_zones = nz;
+  out->zone_rows = hr + nl + na;
+  out->n_lb_misses = nm;
+  out->lb_miss_obj = hr + nl + na + nz;
+  out->lb_miss_j = hr + nl + na + nz + nm;
+  out->lb_miss_name = hs;
+  out->lb_miss_region = hs + nm;
+}
+
 static void do_diff(gar_engine *e, gar_changeset *out, bool to_host, const gar_keyset *ks = nullptr, const gar_bindings *bd = nullptr) {
   if (!e->loaded) throw InvalidError{"no snapshot loaded"};
   CK(cudaSetDevice(e->device));
@@ -1553,33 +1653,11 @@ static void do_diff(gar_engine *e, gar_changeset *out, bool to_host, const gar_k
     rc = P.run(&dc, ops_alloc);
   } else {
     // incremental mode: upload the key batch (rows + deleted keys)
-    if ((ks->n_rows && !ks->rows) || (ks->n_deleted && (!ks->deleted_kind || !ks->deleted_key))) throw InvalidError{"NULL key set arrays"};
-    for (u32 k = 0; k < ks->n_rows; k++)
-      if (ks->rows[k] >= e->T.o.n_objects) throw InvalidError{"key set row out of range"};
     n_out = ks->n_rows;
-    u32 *rows = (u32 *)e->dev_ensure(e->d_key_rows, 4 * (size_t)(ks->n_rows + 1));
-    if (ks->n_rows) CK(cudaMemcpyAsync(rows, ks->rows, 4 * (size_t)ks->n_rows, cudaMemcpyHostToDevice, e->stream));
-    std::vector<u8> slab;
-    std::vector<gar_str> refs(ks->n_deleted);
-    std::vector<u8> kinds(ks->n_deleted);
-    for (u32 k = 0; k < ks->n_deleted; k++) {
-      if (!ks->deleted_key[k] || ks->deleted_kind[k] > GAR_KIND_INGRESS) throw InvalidError{"bad deleted key"};
-      size_t len = strlen(ks->deleted_key[k]);
-      refs[k] = GAR_STR(slab.size(), len);
-      slab.insert(slab.end(), ks->deleted_key[k], ks->deleted_key[k] + len);
-      kinds[k] = ks->deleted_kind[k];
-    }
-    slab.resize(slab.size() + GAR_SLAB_PAD, 0);
-    u8 *dslab = (u8 *)e->dev_ensure(e->d_del_slab, slab.size());
-    u8 *dkind = (u8 *)e->dev_ensure(e->d_del_kind, ks->n_deleted + 1);
-    gar_str *dkey = (gar_str *)e->dev_ensure(e->d_del_key, 8 * (size_t)(ks->n_deleted + 1));
-    CK(cudaMemcpyAsync(dslab, slab.data(), slab.size(), cudaMemcpyHostToDevice, e->stream));
-    if (ks->n_deleted) {
-      CK(cudaMemcpyAsync(dkind, kinds.data(), ks->n_deleted, cudaMemcpyHostToDevice, e->stream));
-      CK(cudaMemcpyAsync(dkey, refs.data(), 8 * (size_t)ks->n_deleted, cudaMemcpyHostToDevice, e->stream));
-    }
-    CK(cudaStreamSynchronize(e->stream));  // the staging vectors go out of scope
-    rc = P.run_keys(rows, ks->n_rows, DelKeys{dkind, dkey, dslab}, ks->n_deleted, &dc, ops_alloc);
+    const u32 *rows;
+    DelKeys D;
+    upload_keyset(e, ks, &rows, &D);
+    rc = P.run_keys(rows, ks->n_rows, D, ks->n_deleted, &dc, ops_alloc);
   }
   if (rc == GAR_OK && e->shard_home && dc.n_ops) e->for_each("shard_translate_ops", (u32)dc.n_ops, FShTranslateOps{(gar_op *)e->d_ops.p, e->sharder->gids});
   CK(cudaEventRecord(e->ev[3], e->stream));
@@ -1794,6 +1872,12 @@ void gar_engine_destroy(gar_engine *e) {
   for (DBuf *b : {&e->cluster_dev, &e->d_status_ga, &e->d_status_r53, &e->d_derived, &e->d_ops, &e->d_tok_code, &e->d_tok_name, &e->d_tok_region,
                   &e->d_dport_begin, &e->d_dports, &e->d_scan_tiles, &e->d_hist})
     cudaFree(b->p);
+  for (auto &b : e->rs_buf) cudaFree(b.p);
+  for (HostReadSet *h : e->free_read_sets) {
+    cudaFreeHost(h->rows.p);
+    cudaFreeHost(h->strs.p);
+    delete h;
+  }
   for (HostResult *h : e->free_results) {
     for (DBuf *b : {&h->status_ga, &h->status_r53, &h->derived, &h->ops, &h->tok_code, &h->tok_name, &h->tok_region, &h->dport_begin, &h->dports, &h->obj_gid}) cudaFreeHost(b->p);
     delete h;
@@ -1846,6 +1930,18 @@ int gar_diff_device(gar_engine *e, gar_changeset *out) {
 int gar_diff_keys(gar_engine *e, const gar_keyset *keys, gar_changeset *out) {
   if (!out || !keys) return GAR_E_INVALID;
   return guarded(e, [&] { do_diff(e, out, true, keys); });
+}
+
+int gar_read_set(gar_engine *e, const gar_keyset *keys, gar_readset *out) {
+  if (!out || !keys) return GAR_E_INVALID;
+  return guarded(e, [&] { do_read_set(e, keys, out); });
+}
+
+void gar_read_set_free(gar_engine *e, gar_readset *rs) {
+  if (!e || !rs) return;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (rs->opaque) e->free_read_sets.push_back((HostReadSet *)rs->opaque);
+  memset(rs, 0, sizeof(*rs));
 }
 
 int gar_bindings_diff(gar_engine *e, const gar_bindings *bindings, gar_changeset *out) {

@@ -1435,3 +1435,172 @@ struct Pipeline {
     return run_with(dc, false, [&] { return decide_bindings(b, ops_alloc); });
   }
 };
+
+// ------------------------------------------------------------------ read set (gar_read_set, include/garecon.h)
+//
+// Backend: for_each, fill32, exclusive_scan(u64 *), download, and read_set_buf(k, bytes) — scratch that no recorded launch
+// sequence holds, so the call grows it without dropping the full diff's graph (the 64-bit scan keeps its own tile states too).
+// Steps: prepare as gar_diff_keys does (Pipeline::run_with) -> items per key, scan -> mark (one thread per item) -> popcount
+// per bitmap word, scan -> emit rows ascending, zeroing every word read: the bitmaps are all zero between calls, so a call
+// costs O(keys + items + table rows / 32).  After a failed call they are cleared again before they are trusted.
+GAR_HD u32 popc32(u32 v) {
+#if defined(__CUDA_ARCH__)
+  return (u32)__popc(v);
+#else
+  return (u32)__builtin_popcount(v);
+#endif
+}
+struct FReadSetCount {
+  DevTables T;
+  Work W;
+  const u32 *rows;
+  u32 m;
+  DelKeys D;
+  Cursor *cur;  // [2 nd]
+  u64 *items;   // [m + nd + 1]
+  GAR_HD void operator()(u32 t) const {
+    if (t < m) items[t] = read_set_row_items(T, W, rows[t]);
+    else items[t] = read_set_deleted_items(W, D.kind[t - m], mkstr(D.slab, D.key[t - m]), cur + 2 * (t - m));
+  }
+};
+struct FReadSetMark {
+  DevTables T;
+  Work W;
+  const u32 *rows;
+  u32 m, nkeys;
+  DelKeys D;
+  const Cursor *cur;
+  const u64 *items;  // exclusive-scanned
+  u64 base;
+  ReadSetBits B;
+  GAR_HD void operator()(u32 x) const {
+    const u64 q = base + x;
+    u32 lo = 0, hi = nkeys;  // the last key whose first item is <= q (a key with no items shares its offset with the next)
+    while (hi - lo > 1) {
+      const u32 mid = (lo + hi) >> 1;
+      if (items[mid] <= q) lo = mid;
+      else hi = mid;
+    }
+    const u32 r = (u32)(q - items[lo]);
+    if (lo < m) read_set_row_item(T, W, B, rows[lo], r);
+    else read_set_deleted_item(T, W, B, D.kind[lo - m], mkstr(D.slab, D.key[lo - m]), cur + 2 * (lo - m), r);
+  }
+};
+struct FReadSetPopc {
+  const u32 *bits;
+  u64 *cnt;
+  GAR_HD void operator()(u32 w) const { cnt[w] = popc32(bits[w]); }
+};
+struct FReadSetSizes {
+  const u64 *cnt;
+  ReadSetBits B;
+  u64 *sizes;  // [RS_N + 1]: the scanned count at the first word of each bitmap, and the total
+  GAR_HD void operator()(u32 s) const { sizes[s] = cnt[B.wb[s]]; }
+};
+struct ReadSetOut {
+  u32 *rows[RS_N];  // ascending rows per bitmap (RS_MISS: lbIngress rows, before the expansion below)
+  u32 *miss_obj, *miss_j;
+  gar_str *miss_name, *miss_region;
+};
+struct FReadSetEmit {
+  DevTables T;
+  Work W;
+  const u64 *cnt;
+  ReadSetBits B;
+  ReadSetOut O;
+  GAR_HD void operator()(u32 w) const {
+    u32 v = B.bits[w];
+    if (!v) return;
+    B.bits[w] = 0;
+    u32 s = 0;
+    while (w >= B.wb[s + 1]) s++;
+    u64 pos = cnt[w] - cnt[B.wb[s]];
+    for (; v; v &= v - 1, pos++) {
+      const u32 r = (w - B.wb[s]) * 32 + ctz64(v);
+      if (s != RS_MISS) {
+        O.rows[s][pos] = r;
+        continue;
+      }
+      u32 lo = 0, hi = T.o.n_objects;  // the object row whose lbIngress range holds r
+      while (hi - lo > 1) {
+        const u32 mid = (lo + hi) >> 1;
+        if (T.o.obj_lbi_begin[mid] <= r) lo = mid;
+        else hi = mid;
+      }
+      O.miss_obj[pos] = lo;
+      O.miss_j[pos] = r - T.o.obj_lbi_begin[lo];
+      O.miss_name[pos] = W.tok_name[r];
+      O.miss_region[pos] = W.tok_region[r];
+    }
+  }
+};
+
+// the bitmap buffer last cleared and how many of its words are known to be zero; kept by the engine between calls
+struct ReadSetClean {
+  u32 *bits = nullptr;
+  u32 words = 0;
+};
+template <class Be, class Pipe>
+struct ReadSetter {
+  Be &be;
+  Pipe &P;
+  ReadSetClean &clean;
+  enum { RB_ITEMS, RB_CUR, RB_BITS, RB_CNT, RB_SIZES, RB_OUT32, RB_OUT64, RB_N };
+  // rows of each bitmap (RS_N) and the size of each, device pointers valid until the next call
+  ReadSetOut out;
+  u32 n[RS_N];
+  int run(const u32 *rows, u32 m, DelKeys D, u32 nd) {
+    DiffCounts dc{};
+    int rc = P.run_with(&dc, false, [&] {
+      if (nd) P.build_owner_indexes();
+      return GAR_OK;
+    });
+    if (rc != GAR_OK) return rc;
+    const DevTables &T = P.T;
+    const Work &W = P.W;
+    const u32 nk = m + nd;
+    u64 *items = (u64 *)be.read_set_buf(RB_ITEMS, 8 * ((size_t)nk + 2));
+    Cursor *cur = (Cursor *)be.read_set_buf(RB_CUR, sizeof(Cursor) * (2 * (size_t)nd + 1));
+    const u32 size[RS_N] = {T.a.n_lbs, T.a.n_accels, T.a.n_zones, T.o.n_lbi};
+    ReadSetBits B;
+    B.wb[0] = 0;
+    for (int s = 0; s < RS_N; s++) B.wb[s + 1] = B.wb[s] + (size[s] + 31) / 32;
+    const u32 nw = B.wb[RS_N];
+    B.bits = (u32 *)be.read_set_buf(RB_BITS, 4 * ((size_t)nw + 1));
+    if (B.bits != clean.bits || nw > clean.words) be.fill32(B.bits, 0, nw);  // a new buffer, or the last call did not finish
+    clean.bits = B.bits;
+    clean.words = 0;
+
+    if (nk) be.for_each("read_set_count", nk, FReadSetCount{T, W, rows, m, D, cur, items});
+    be.fill32((u32 *)(items + nk), 0, 2);
+    be.exclusive_scan(items, nk + 1);
+    u64 total = 0;
+    be.download(&total, items + nk, 8);
+    constexpr u64 CHUNK = 1ull << 30;
+    for (u64 b = 0; b < total; b += CHUNK)
+      be.for_each("read_set_mark", (u32)(total - b < CHUNK ? total - b : CHUNK), FReadSetMark{T, W, rows, m, nk, D, cur, items, b, B});
+
+    u64 *cnt = (u64 *)be.read_set_buf(RB_CNT, 8 * ((size_t)nw + 2));
+    u64 *sizes = (u64 *)be.read_set_buf(RB_SIZES, 8 * (RS_N + 1));
+    if (nw) be.for_each("read_set_popcount", nw, FReadSetPopc{B.bits, cnt});
+    be.fill32((u32 *)(cnt + nw), 0, 2);
+    be.exclusive_scan(cnt, nw + 1);
+    be.for_each("read_set_sizes", RS_N + 1, FReadSetSizes{cnt, B, sizes});
+    u32 *o32 = (u32 *)be.read_set_buf(RB_OUT32, 4 * ((size_t)size[0] + size[1] + size[2] + 2 * (size_t)size[3] + 1));
+    gar_str *o64 = (gar_str *)be.read_set_buf(RB_OUT64, 8 * (2 * (size_t)size[3] + 1));
+    out.rows[RS_LB] = o32;
+    out.rows[RS_ACC] = o32 + size[0];
+    out.rows[RS_ZONE] = out.rows[RS_ACC] + size[1];
+    out.rows[RS_MISS] = nullptr;
+    out.miss_obj = out.rows[RS_ZONE] + size[2];
+    out.miss_j = out.miss_obj + size[3];
+    out.miss_name = o64;
+    out.miss_region = o64 + size[3];
+    if (nw) be.for_each("read_set_emit", nw, FReadSetEmit{T, W, cnt, B, out});
+    u64 sz[RS_N + 1];
+    be.download(sz, sizes, sizeof(sz));
+    for (int s = 0; s < RS_N; s++) n[s] = (u32)(sz[s + 1] - sz[s]);
+    clean.words = nw;
+    return GAR_OK;
+  }
+};

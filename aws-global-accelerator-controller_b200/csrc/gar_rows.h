@@ -536,27 +536,31 @@ struct OwnerIter {
   Str key;
 };
 GAR_HD OwnerIter owner_open(const Work &W, u64 key_hash, Str key) { return OwnerIter{idx_open(W.ix_owner, key_hash), key}; }
+GAR_HD bool owner_match(const DevTables &T, const IdxEntry &e, u32 kind, Str key) {
+  return ((((e.a0 & ACC_OWNER_INGRESS) != 0) ? 1u : 0u) == kind) && streq(mkstr(T.a.slab, e.s0), key);
+}
 GAR_HD u32 owner_next(const DevTables &T, const Work &W, u32 kind, OwnerIter &it) {
   IdxEntry e;
-  while (idx_next(W.ix_owner, it.c, &e)) {
-    if ((((e.a0 & ACC_OWNER_INGRESS) != 0) ? 1u : 0u) != kind) continue;
-    if (streq(mkstr(T.a.slab, e.s0), it.key)) return e.row;
-  }
+  while (idx_next(W.ix_owner, it.c, &e))
+    if (owner_match(T, e, kind, it.key)) return e.row;
   return GAR_NONE;
 }
 
 // ListGlobalAcceleratorByHostname (global_accelerator.go:62-85): number of matches (saturating at 2), the first
-// match and its DnsName ref
-GAR_HD u32 find_by_hostname(const DevTables &T, const Work &W, Str hostname, u32 *first, gar_str *first_dns) {
+// match and its DnsName ref (and, for the read set, the second match)
+GAR_HD u32 find_by_hostname(const DevTables &T, const Work &W, Str hostname, u32 *first, gar_str *first_dns, u32 *second = nullptr) {
   Cursor c = idx_open(W.ix_thost, key_hash_str(hostname));
   u32 n = 0;
   *first = GAR_NONE;
+  if (second) *second = GAR_NONE;
   IdxEntry e;
   while (idx_next(W.ix_thost, c, &e)) {
     if (!streq(mkstr(T.a.slab, e.s0), hostname)) continue;
     if (n == 0) {
       *first = e.row;
       *first_dns = e.s1;
+    } else if (second) {
+      *second = e.row;
     }
     if (++n >= 2) break;
   }
@@ -1863,4 +1867,81 @@ GAR_HD u32 egb_reconcile(const DevTables &T, const Work &W, const DevBindings &B
     }
   s.put(H(GAR_OP_EGB_UPDATE_STATUS), k, 0, GAR_NONE, GAR_NONE, GAR_NONE);
   return GAR_STATUS(GAR_ST_OK, 0, 0);
+}
+
+// ------------------------------------------------------------------ read set (gar_read_set)
+//
+// The resident AWS rows that the decisions of a keyset read, by the rules of include/garecon.h "gar_read_set", as bits in four
+// bitmaps kept back to back (load balancers, accelerators, zones, lbIngress rows whose load balancer is missing).  A key's work
+// is flattened into items so that a hot owner's lists (10^5 accelerators or owner values) spread over the grid instead of one
+// thread or one warp (DESIGN.md §4 "Skew"):
+//   object row i   one item per lbIngress, one per entry of its owned-accelerator segment, one per entry of its owned-value
+//                  segment, one for the pieces of its route53-hostname annotation;
+//   deleted key    one item per entry of its ix_owner bucket, one per entry of its ix_val bucket (the walks FDelKeyGa and
+//                  FDelKeyR53 make; a tag and key compare per entry decides).
+enum { RS_LB = 0, RS_ACC = 1, RS_ZONE = 2, RS_MISS = 3, RS_N = 4 };
+struct ReadSetBits {
+  u32 *bits;
+  u32 wb[RS_N + 1];  // first word of each bitmap; wb[RS_N] = the total
+};
+GAR_HD void rs_mark(const ReadSetBits &B, u32 s, u32 row) {
+  const u32 b = B.wb[s] * 32 + row, m = 1u << (b & 31);
+#if defined(__CUDA_ARCH__)
+  u32 *w = B.bits + (b >> 5);
+  if (!(__ldcg(w) & m)) atomicOr(w, m);  // a hot zone's word is read far more often than it is written
+#else
+  B.bits[b >> 5] |= m;
+#endif
+}
+GAR_HD u32 read_set_row_items(const DevTables &T, const Work &W, u32 i) {
+  const OwnRange a = own_accs(W, i), v = own_vals(W, i);
+  return (T.o.obj_lbi_begin[i + 1] - T.o.obj_lbi_begin[i]) + (a.end - a.pos) + (v.end - v.pos) + 1;
+}
+GAR_HD void read_set_row_item(const DevTables &T, const Work &W, const ReadSetBits &B, u32 i, u32 q) {
+  const u32 jb = T.o.obj_lbi_begin[i], nj = T.o.obj_lbi_begin[i + 1] - jb;
+  if (q < nj) {
+    const u32 p = jb + q;
+    if (W.tok_code[p] > GAR_TOK_NLB) return;  // PANIC / NOT_AWS / ERR_*: the decisions stop or skip before any lookup
+    u32 st;
+    const u32 lb = find_lb(T, W, mkstr(T.o.slab, W.tok_region[p]), mkstr(T.o.slab, W.tok_name[p]), &st);
+    if (lb != GAR_NONE) rs_mark(B, RS_LB, lb);
+    else rs_mark(B, RS_MISS, p);
+    u32 a0, a1;
+    gar_str dns;
+    find_by_hostname(T, W, mkstr(T.o.slab, T.o.lbi_hostname[p]), &a0, &dns, &a1);  // the Route53 count gate reads two
+    if (a0 != GAR_NONE) rs_mark(B, RS_ACC, a0);
+    if (a1 != GAR_NONE) rs_mark(B, RS_ACC, a1);
+    return;
+  }
+  q -= nj;
+  const OwnRange a = own_accs(W, i);
+  if (q < a.end - a.pos) return rs_mark(B, RS_ACC, W.own[a.pos + q].row);
+  q -= a.end - a.pos;
+  const OwnRange v = own_vals(W, i);
+  if (q < v.end - v.pos) return rs_mark(B, RS_ZONE, owned_hit(load_entry(W.own + v.pos + q)).zone);
+  if (!(W.derived[i] & GAR_DV_R53_ANNOTATED)) return;
+  const Str all = mkstr(T.o.slab, W.ann_r53[i]);
+  u32 pos = 0;
+  Str piece;
+  while (next_piece(all, &pos, &piece)) {  // strings.Split(annotation, ","); a piece without a zone adds nothing
+    const u32 z = find_hosted_zone(T, W, piece);
+    if (z != GAR_NONE) rs_mark(B, RS_ZONE, z);
+  }
+}
+// a deleted key's two buckets: [0] ix_owner, [1] ix_val (one key hash, so one tag)
+GAR_HD u32 read_set_deleted_items(const Work &W, u32 kind, Str key, Cursor *c) {
+  const u64 h = key_hash_kinded(kind, key);
+  c[0] = idx_open(W.ix_owner, h);
+  c[1] = idx_open(W.ix_val, h);
+  return (c[0].end - c[0].pos) + (c[1].end - c[1].pos);
+}
+GAR_HD void read_set_deleted_item(const DevTables &T, const Work &W, const ReadSetBits &B, u32 kind, Str key, const Cursor *c, u32 q) {
+  const u32 no = c[0].end - c[0].pos;
+  if (q < no) {
+    const IdxEntry e = load_entry(W.ix_owner.ent + c[0].pos + q);
+    if (e.tag == c[0].tag && owner_match(T, e, kind, key)) rs_mark(B, RS_ACC, e.row);
+    return;
+  }
+  const IdxEntry e = load_entry(W.ix_val.ent + c[1].pos + (q - no));
+  if (e.tag == c[1].tag && owned_match(T, e, kind, key)) rs_mark(B, RS_ZONE, owned_hit(e).zone);
 }

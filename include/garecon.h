@@ -387,6 +387,51 @@ typedef struct gar_keyset {
 } gar_keyset;
 int gar_diff_keys(gar_engine *e, const gar_keyset *keys, gar_changeset *out);
 
+/* Read set: the resident AWS rows that the decisions of a keyset read, so that a worker fed by deltas can re-describe exactly
+   those rows (as gar_snapshot_apply_actual input) before it calls gar_diff_keys on the same keyset.  The reference re-lists AWS
+   inside every reconcile; a resident snapshot only sees what the worker re-lists, and this call says what that must be.
+   The units are gar_actual_delta's: an LB row, an accelerator with its whole subtree, a zone with its whole record list.
+   Rules (a superset of what gar_diff_keys reads, independent of which branch each decision takes):
+     - for each row i of keys->rows and each lbIngress j of i whose tokeniser code is GAR_TOK_ALB_INTERNAL, GAR_TOK_ALB_PUBLIC or
+       GAR_TOK_NLB: the first LB row with that (region, name), or a miss entry when there is none; and the first two accelerators
+       of this cluster (managed, cluster tag) whose target-hostname tag equals the lbIngress hostname (what the Route53 count
+       gate reads);
+     - for each row i: every accelerator of its owned-accelerator list (the list of the lowest row with i's key, as the decisions
+       read it); the zone of every owner value of its key; and the zone GetHostedZone finds for every piece of
+       strings.Split(route53-hostname annotation, ",") — a piece without a zone adds nothing (a new zone arrives through the
+       worker's ListHostedZones comparison and gar_snapshot_apply_zones);
+     - for each deleted key: the accelerators its cleanup deletes (owner tag of the key) and the zones of the owner values its
+       Route53 cleanup finds.
+   Guarantee: change any resident row outside the set, in any column that does not decide membership (LB region and name,
+   accelerator tags, zone name, record values that are an owner value of a key in the set), apply it with
+   gar_snapshot_apply_actual, and gar_diff_keys of the same keyset returns the identical change set (when a replaced subtree or
+   record list changes its number of children, the listener, endpoint-group, record and value rows the ops name are renumbered
+   by the new layout, nothing else).
+   Limitation: a resource that becomes owned out of band (an accelerator whose tags are edited to name a key, a record given an
+   owner value) is outside the set until it is listed; the periodic full re-list covers it.
+   Validation is gar_diff_keys' (rows < n_objects, deleted keys a kind plus a NUL-terminated "ns/name"); GAR_E_INVALID changes
+   nothing.  GAR_E_STATE before a load and on a sharded sub-snapshot (or once gar_shard_route has run on the loaded slice).  An
+   attached snapshot is allowed.  The call prepares a stale snapshot exactly as gar_diff_keys would (the object side after an
+   object delta or compaction, everything after an AWS or zone delta, ix_owner / ix_val when deleted keys need them); it changes
+   nothing resident and leaves the recorded launch sequence as gar_diff_keys does: the next full diff replays if it would have.
+   The arrays are engine-owned pinned host memory, valid until gar_read_set_free. */
+typedef struct gar_readset {
+  uint32_t n_lbs;
+  const uint32_t *lb_rows;         /* [n_lbs] ascending, distinct resident LB rows */
+  uint32_t n_lb_misses;            /* probes that found no LB row, ascending by (row, j), one per lbIngress: */
+  const uint32_t *lb_miss_obj;     /*   [n_lb_misses] object row */
+  const uint32_t *lb_miss_j;       /*   [n_lb_misses] lbIngress index within the object */
+  const gar_str *lb_miss_name;     /*   [n_lb_misses] tokenised LB name, and */
+  const gar_str *lb_miss_region;   /*   [n_lb_misses] region: refs into the resident object slab (gar_snapshot_read_slab) */
+  uint32_t n_accels;
+  const uint32_t *acc_rows;        /* [n_accels] ascending, distinct resident accelerator rows (whole subtrees) */
+  uint32_t n_zones;
+  const uint32_t *zone_rows;       /* [n_zones] ascending, distinct resident zone rows (whole record lists) */
+  void *opaque;                    /* engine-private; do not touch */
+} gar_readset;
+int gar_read_set(gar_engine *e, const gar_keyset *keys, gar_readset *out);
+void gar_read_set_free(gar_engine *e, gar_readset *rs);
+
 /* ---------------------------------------------------------------- object deltas: keeping the resident snapshot current
    Informer events (add / update / delete of a Service or Ingress) applied to the loaded object table on the device, so that
    gar_diff_keys (and gar_diff, gar_bindings_diff) see them without a reload.  The AWS tables are left as loaded.
