@@ -286,3 +286,30 @@ GAR_HD bool idx_next(const HashIdx &ix, Cursor &c, IdxEntry *out) {
   }
   return false;
 }
+// A cursor whose next entry is loaded when it is opened: a row that opens several of them issues every bucket's bounds and
+// first entry before it walks any bucket, so the probe chains overlap.  idx_next over it yields exactly what it yields over a
+// Cursor; the entry after a hit is loaded only when the walk goes on.
+struct PreCursor {
+  Cursor c;
+  IdxEntry e;  // the entry at c.pos, once `loaded`
+  bool loaded;
+};
+GAR_HD PreCursor idx_open_pre(const HashIdx &ix, u64 h) {
+  PreCursor p;
+  p.c = idx_open(ix, h);
+  p.loaded = p.c.pos < p.c.end;
+  if (p.loaded) p.e = load_entry(ix.ent + p.c.pos);
+  return p;
+}
+GAR_HD bool idx_next(const HashIdx &ix, PreCursor &p, IdxEntry *out) {
+  while (p.c.pos < p.c.end) {
+    if (!p.loaded) p.e = load_entry(ix.ent + p.c.pos);
+    p.loaded = false;
+    p.c.pos++;
+    if (p.e.tag == p.c.tag) {
+      *out = p.e;
+      return true;
+    }
+  }
+  return false;
+}

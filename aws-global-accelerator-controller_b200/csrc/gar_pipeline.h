@@ -49,7 +49,7 @@ enum Slot {
   S_SORT_KEYS = S_IX_OVN + 3, S_SORT_VALS, S_SORT_KEYS_ALT, S_SORT_VALS_ALT, S_SORT_TAGS,
   S_COUNTS, S_STATUS_GA, S_STATUS_R53, S_OPS, S_ERRFLAG, S_IX_EG, S_IX_EG_ENT, S_IX_EG_PAD,
   S_VAL_OBJ, S_ACC_OBJ, S_OBJ_CANON, S_OWN_BEGIN, S_OWN_FILL, S_OWN_ENT, S_OWN_MULTI,
-  S_IXA_BEGIN, S_IXA_FILL, S_IXA_ENT, S_IXA_MULTI, S_OVN_FILL, S_OVN_MULTI, S_LB_HASH, S_REC_FLAGS,
+  S_IXA_BEGIN, S_IXA_FILL, S_IXA_ENT, S_IXA_MULTI, S_OVN_FILL, S_OVN_MULTI, S_LB_HASH, S_REC_FLAGS, S_LBI_RES,
   S_NSLOTS
 };
 
@@ -571,6 +571,13 @@ struct FResolveAccel {
   Work W;
   GAR_HD void operator()(u32 a) const { resolve_accel(T, W, a); }
 };
+// the load balancer and target-hostname accelerators of each lbIngress row (lbi_resolve): they read the object side's
+// tokens and the AWS side's indexes, so they run in both forms of the owner-keyed joins, which follow every change to either
+struct FLbiResolve {
+  DevTables T;
+  Work W;
+  GAR_HD void operator()(u32 r) const { lbi_resolve(T, W, r); }
+};
 // owned-list records (payloads: gar_rows.h "index probes"): x < nacc is accelerator x, else owner value x - nacc
 GAR_HD IdxEntry own_entry(const DevTables &T, const Work &W, u32 x) {
   IdxEntry e;
@@ -954,6 +961,7 @@ struct Pipeline {
     W.tok_code = (u8 *)be.out_tok_code(nlbi);
     W.tok_name = (gar_str *)be.out_tok_name(nlbi);
     W.tok_region = (gar_str *)be.out_tok_region(nlbi);
+    W.lbi_res = (LbiRes *)be.ensure(S_LBI_RES, sizeof(LbiRes) * (size_t)(nlbi + 1));
     W.r53_mode = (u8 *)be.ensure(S_R53_MODE, (size_t)n + 1);
     W.r53_acc = (u32 *)be.ensure(S_R53_ACC, 4 * (size_t)(n + 1));
     W.r53_acc_dns = (gar_str *)be.ensure(S_R53_ACC_DNS, 8 * (size_t)(n + 1));
@@ -1076,6 +1084,8 @@ struct Pipeline {
   // (alias links when `link_aliases`, object row, orphan mark) and owner-keyed accelerators (object row) counts the owned-list
   // segments and the buckets of the orphan-value index, whose keys exist only now; then both are built the way group A is:
   // one scan each, one fused placement through cursors, ordering of the segments / buckets with two or more rows.
+  // The same launch resolves every lbIngress row's load balancer and target-hostname accelerators (lbi_res): like the owner
+  // joins they read both sides of the snapshot, and this is the one step that follows every change to either side.
   void resolve_owners(bool link_aliases) {
     const u32 n = T.o.n_objects, nacc = T.a.n_accels, nval = T.a.n_values, nseg = 2 * n;
     u32 *overflow = errflag + FW_IDX_OVERFLOW;
@@ -1090,8 +1100,9 @@ struct Pipeline {
     } else {
       W.hist[IX_OVN] = IxHist{nullptr, 0};
     }
-    if (link_aliases) be.for_each_multi("value_joins", {nval, nacc}, FValueJoins{T, W}, FResolveAccel{T, W});
-    else be.for_each_multi("resolve_owners", {nval, nacc}, FResolveValue{T, W}, FResolveAccel{T, W});
+    const u32 nlbi = T.o.n_lbi;
+    if (link_aliases) be.for_each_multi("value_joins", {nval, nacc, nlbi}, FValueJoins{T, W}, FResolveAccel{T, W}, FLbiResolve{T, W});
+    else be.for_each_multi("resolve_owners", {nval, nacc, nlbi}, FResolveValue{T, W}, FResolveAccel{T, W}, FLbiResolve{T, W});
     be.exclusive_scan(W.own_begin, nseg + 1);  // [nseg] = number of records
     IdxEntry *own = (IdxEntry *)be.ensure(S_OWN_ENT, sizeof(IdxEntry) * ((size_t)nacc + nval + 1));
     if (!force_radix) {
@@ -1172,6 +1183,7 @@ struct Pipeline {
   bool tiny_caps = false;  // test hook (environment GAR_TINY_CAPS=1): start every capacity at 1 so that the grow-and-rerun paths run
   int prepare() {
     const u32 n = T.o.n_objects, nacc = T.a.n_accels, nzone = T.a.n_zones, nrec = T.a.n_records;
+    if (T.a.n_lbs > LBI_ROW_MASK || nacc > LBI_ROW_MASK) return GAR_E_INVALID;  // LbiRes keeps these rows in 30 bits
     alloc_work();
     if (!force_radix) arm_group_a((1u << IX_LB) | (1u << IX_THOST) | (1u << IX_ZONE) | (1u << IX_ALIAS) | (1u << IX_OBJ));
     stage1();
@@ -1212,8 +1224,8 @@ struct Pipeline {
   //                value -> alias links and the on-demand ix_owner / ix_val: depend on the AWS tables only and stay resident
   //                across deltas;
   //   object side  classify, tokenise, listen ports, ix_obj + obj_canon, and the owner-keyed joins that point into the object
-  //                rows (val_obj / acc_obj, the owned lists, the orphan value marks + ix_ovn): rebuilt over the whole resident
-  //                table after a delta.
+  //                rows (val_obj / acc_obj, the owned lists, the orphan value marks + ix_ovn) and the lbIngress rows (lbi_res):
+  //                rebuilt over the whole resident table after a delta.
   // obj_stale: the object table changed since the object side was built.  owners_stale: the owner-keyed joins lag behind ix_obj.
   bool obj_stale = false, owners_stale = false;
   void prepare_objects() {

@@ -73,6 +73,22 @@ struct alignas(16) ValLink {  // per owner value row: first alias A record under
   u32 alias_row, pad;
   gar_str alias_dns;
 };
+// Both AWS-side lookups of one lbIngress row (lbi_resolve), resolved once per snapshot state and read by the decide kernels in
+// place of their own probes.  One 32-byte sector per row.  Filled for rows whose tokeniser code is ALB or NLB only.
+struct alignas(32) LbiRes {
+  u32 lb;          // GetLoadBalancer: first ix_lb row of (region, name) | LBI_* << 30; GAR_NONE (= LBI_NOT_FOUND) when there is none
+  u32 acc;         // ListGlobalAcceleratorByHostname: first ix_thost row of the hostname | match count (saturating at 2) << 30
+  gar_str acc_dns; // DnsName of that first accelerator (0 without a match)
+  gar_str lb_dns;  // DNSName and ARN of the load balancer (0 when not found)
+  gar_str lb_arn;
+};
+// the verdict of EnsureGlobalAcceleratorFor*'s load-balancer checks (global_accelerator.go:112-140), in the order they run
+enum { LBI_OK = 0, LBI_DNS_MISMATCH = 1, LBI_NOT_ACTIVE = 2, LBI_NOT_FOUND = 3 };
+#define LBI_ROW_MASK 0x3FFFFFFFu  // rows of a snapshot stay below 2^30 (Pipeline::prepare refuses larger tables)
+GAR_HD u32 lbi_verdict(const LbiRes &r) { return r.lb >> 30; }
+GAR_HD u32 lbi_lb(const LbiRes &r) { return r.lb == GAR_NONE ? GAR_NONE : r.lb & LBI_ROW_MASK; }
+GAR_HD u32 lbi_acc_count(const LbiRes &r) { return r.acc >> 30; }
+GAR_HD u32 lbi_acc(const LbiRes &r) { return lbi_acc_count(r) ? r.acc & LBI_ROW_MASK : GAR_NONE; }
 
 // the hash indexes, in build order (group A is built together in one pass, IX_OVN after the per-value joins)
 enum IxId { IX_LB, IX_OWNER, IX_THOST, IX_ZONE, IX_VAL, IX_ALIAS, IX_OBJ, IX_OVN, IX_N };
@@ -109,6 +125,7 @@ struct Work {
   // lbIngress rows
   u8 *tok_code;
   gar_str *tok_name, *tok_region;
+  LbiRes *lbi_res;  // [n_lbi] load balancer + target-hostname accelerators (lbi_resolve, run with the owner-keyed joins)
   // accelerators
   u32 *acc_flags;
   gar_str *acc_owner_key;  // owner tag value minus the "service/" | "ingress/" prefix (refs into actual slab)
@@ -504,9 +521,10 @@ GAR_HD void classify_value(const DevTables &T, const Work &W, u32 v) { classify_
 //   accelerator segment  row=accel
 //   value segment        row=value a0=record  a1=zone|backslash  tag=first alias A record row  s0=its alias DNS ref  s1=record name ref
 
-// GetLoadBalancer (load_balancer.go:13-30) on a client bound to `region` (aws.go:23-25): first row wins
-GAR_HD u32 find_lb(const DevTables &T, const Work &W, Str region, Str name, u32 *state) {
-  Cursor c = idx_open(W.ix_lb, key_hash_lb(region, name));
+// GetLoadBalancer (load_balancer.go:13-30) on a client bound to `region` (aws.go:23-25): first row wins.  The walk takes an
+// opened ix_lb cursor (Cursor or PreCursor).
+template <class C>
+GAR_HD u32 lb_walk(const DevTables &T, const Work &W, C &c, Str region, Str name, u32 *state) {
   IdxEntry e;
   while (idx_next(W.ix_lb, c, &e))
     if (streq(mkstr(T.a.slab, e.s0), name) && streq(mkstr(T.a.slab, e.s1), region)) {
@@ -514,6 +532,10 @@ GAR_HD u32 find_lb(const DevTables &T, const Work &W, Str region, Str name, u32 
       return e.row;
     }
   return GAR_NONE;
+}
+GAR_HD u32 find_lb(const DevTables &T, const Work &W, Str region, Str name, u32 *state) {
+  Cursor c = idx_open(W.ix_lb, key_hash_lb(region, name));
+  return lb_walk(T, W, c, region, name, state);
 }
 
 // ListGlobalAcceleratorByResource (global_accelerator.go:87-110) of an object in the cache: its canonical row's accelerator
@@ -547,9 +569,9 @@ GAR_HD u32 owner_next(const DevTables &T, const Work &W, u32 kind, OwnerIter &it
 }
 
 // ListGlobalAcceleratorByHostname (global_accelerator.go:62-85): number of matches (saturating at 2), the first
-// match and its DnsName ref (and, for the read set, the second match)
-GAR_HD u32 find_by_hostname(const DevTables &T, const Work &W, Str hostname, u32 *first, gar_str *first_dns, u32 *second = nullptr) {
-  Cursor c = idx_open(W.ix_thost, key_hash_str(hostname));
+// match and its DnsName ref (and, for the read set, the second match).  The walk takes an opened ix_thost cursor.
+template <class C>
+GAR_HD u32 thost_walk(const DevTables &T, const Work &W, C &c, Str hostname, u32 *first, gar_str *first_dns, u32 *second = nullptr) {
   u32 n = 0;
   *first = GAR_NONE;
   if (second) *second = GAR_NONE;
@@ -565,6 +587,37 @@ GAR_HD u32 find_by_hostname(const DevTables &T, const Work &W, Str hostname, u32
     if (++n >= 2) break;
   }
   return n;
+}
+GAR_HD u32 find_by_hostname(const DevTables &T, const Work &W, Str hostname, u32 *first, gar_str *first_dns, u32 *second = nullptr) {
+  Cursor c = idx_open(W.ix_thost, key_hash_str(hostname));
+  return thost_walk(T, W, c, hostname, first, first_dns, second);
+}
+
+// Both lookups of lbIngress row r that the Global Accelerator and Route53 decisions make (EnsureGlobalAcceleratorFor*,
+// global_accelerator.go:112-140; ensureRoute53, route53.go:56-80).  They read the row's hostname and tokens and the AWS side
+// only, so they are resolved once per snapshot state (Pipeline::resolve_owners).  Both keys are hashed and both buckets'
+// bounds and first entries loaded before either bucket is walked, so the two probe chains overlap.
+GAR_HD void lbi_resolve(const DevTables &T, const Work &W, u32 r) {
+  if (W.tok_code[r] > GAR_TOK_NLB) return;  // no lookup happens for this row: the record is never read
+  const gar_actual &A = T.a;
+  const Str host = mkstr(T.o.slab, T.o.lbi_hostname[r]);
+  const Str region = mkstr(T.o.slab, W.tok_region[r]), name = mkstr(T.o.slab, W.tok_name[r]);
+  PreCursor cl = idx_open_pre(W.ix_lb, key_hash_lb(region, name)), ch = idx_open_pre(W.ix_thost, key_hash_str(host));
+  LbiRes res;
+  u32 state = 0;
+  const u32 lb = lb_walk(T, W, cl, region, name, &state);
+  res.lb_dns = lb != GAR_NONE ? A.lb_dns[lb] : 0;  // in flight while the hostname bucket is walked
+  res.lb_arn = lb != GAR_NONE ? A.lb_arn[lb] : 0;
+  u32 acc = GAR_NONE;
+  res.acc_dns = 0;
+  const u32 nacc = thost_walk(T, W, ch, host, &acc, &res.acc_dns);
+  res.acc = (nacc << 30) | (acc & LBI_ROW_MASK);
+  res.lb = GAR_NONE;
+  if (lb != GAR_NONE) {
+    const u32 v = !streq(mkstr(A.slab, res.lb_dns), host) ? LBI_DNS_MISMATCH : state != GAR_LB_ACTIVE ? LBI_NOT_ACTIVE : LBI_OK;
+    res.lb = (v << 30) | lb;
+  }
+  W.lbi_res[r] = res;
 }
 
 // GetHostedZone (route53.go:335-358) + parentDomain (:383-386)
@@ -632,44 +685,6 @@ GAR_HD bool u_bucket_step(const HashIdx &ix, bool searching, Cursor &c, IdxEntry
   return false;
 }
 #define U_BUCKET_LOOP(searching_expr, cur) for (; GAR_ANY((searching_expr) && (cur).pos < (cur).end);)
-
-// first LB row matching (region, name)  (GetLoadBalancer, load_balancer.go:13-30)
-GAR_HD u32 u_find_lb(const DevTables &T, const Work &W, bool active, Str region, Str name, u32 *state) {
-  u64 h = hmix(u_hash(active, region), u_hash(active, name));
-  Cursor c = u_open(W.ix_lb, active, h);
-  u32 found = GAR_NONE;
-  U_BUCKET_LOOP(found == GAR_NONE, c) {
-    IdxEntry e;
-    bool hit = u_bucket_step(W.ix_lb, found == GAR_NONE, c, &e);
-    bool eq = u_streq(hit, mkstr(T.a.slab, e.s0), name);
-    eq = u_streq(eq, mkstr(T.a.slab, e.s1), region);
-    if (eq) {
-      found = e.row;
-      *state = e.a0;
-    }
-  }
-  return found;
-}
-
-// accelerators whose target-hostname tag equals `hostname` (ListGlobalAcceleratorByHostname, :62-85):
-// count (saturating at 2), first row, its DnsName
-GAR_HD u32 u_find_by_hostname(const DevTables &T, const Work &W, bool active, Str hostname, u32 *first, gar_str *first_dns) {
-  Cursor c = u_open(W.ix_thost, active, u_hash(active, hostname));
-  u32 n = 0;
-  *first = GAR_NONE;
-  U_BUCKET_LOOP(n < 2, c) {
-    IdxEntry e;
-    bool hit = u_bucket_step(W.ix_thost, n < 2, c, &e);
-    if (u_streq(hit, mkstr(T.a.slab, e.s0), hostname)) {
-      if (n == 0) {
-        *first = e.row;
-        *first_dns = e.s1;
-      }
-      n++;
-    }
-  }
-  return n;
-}
 
 // GetHostedZone (route53.go:335-358): one voted round per candidate suffix
 GAR_HD u32 u_find_hosted_zone(const DevTables &T, const Work &W, bool active, Str hostname) {
@@ -898,7 +913,9 @@ GAR_HD void put_delete_chain(const DevTables &T, OpSink &s, u32 obj, u32 kind, u
 
 // acceleratorChanged (global_accelerator.go:412-437), all lanes together.  The rare tags-annotation overlay keeps the
 // scalar routine (divergent, no votes inside).
-GAR_HD bool u_accelerator_changed(const DevTables &T, const Work &W, bool act, u32 i, u32 dv, u32 kind, u32 acc, const AccDigest &d, Str okey, Str lb_dns) {
+// thost_eq: the caller already knows that the accelerator's target-hostname tag equals lb_dns byte for byte (the compare is skipped)
+GAR_HD bool u_accelerator_changed(const DevTables &T, const Work &W, bool act, u32 i, u32 dv, u32 kind, u32 acc, const AccDigest &d, Str okey, Str lb_dns,
+                                  bool thost_eq) {
   const gar_actual &A = T.a;
   bool ch = act && !(d.flags & ACCD_ENABLED);
   // name: the annotation when non-empty, else resource-ns-name
@@ -924,7 +941,8 @@ GAR_HD bool u_accelerator_changed(const DevTables &T, const Work &W, bool act, u
   if (sys && !(fl & ACCD_MANAGED_TRUE)) ch = true;
   // the owner tag equals resource/ns/name: guaranteed by the value pass that put `acc` on this object's list (kind + key compared there)
   bool th = sys && !ch;
-  bool th_eq = u_streq(th, th ? mkstr(A.slab, d.thost) : Str{A.slab, 0}, lb_dns);
+  bool th_cmp = th && !thost_eq;
+  bool th_eq = u_streq(th_cmp, th_cmp ? mkstr(A.slab, d.thost) : Str{A.slab, 0}, lb_dns) || (th && thost_eq);
   if (th && !th_eq) ch = true;
   return ch;
 }
@@ -1008,7 +1026,6 @@ GAR_HD u32 ga_reconcile(const DevTables &T, const Work &W, u32 i, bool valid, Op
     bool act = ensure && !stop && j < nj;
     if (!GAR_ANY(act)) break;
     bool probe = false;
-    Str hostname{o.slab, 0}, tregion{o.slab, 0}, tname{o.slab, 0};
     if (act) {
       u32 code = W.tok_code[jb + j];
       if (code == GAR_TOK_PANIC) {
@@ -1020,39 +1037,38 @@ GAR_HD u32 ga_reconcile(const DevTables &T, const Work &W, u32 i, bool valid, Op
         stop = true;
       } else {
         probe = true;
-        hostname = mkstr(o.slab, o.lbi_hostname[jb + j]);
-        tregion = mkstr(o.slab, W.tok_region[jb + j]);
-        tname = mkstr(o.slab, W.tok_name[jb + j]);
       }
     }
-    // EnsureGlobalAcceleratorFor* (global_accelerator.go:112-211)
-    u32 lb_state = 0;
-    u32 lb = u_find_lb(T, W, probe, tregion, tname, &lb_state);
-    bool have_lb = probe && lb != GAR_NONE;
-    Str lb_dns = have_lb ? mkstr(A.slab, A.lb_dns[lb]) : Str{A.slab, 0};
-    bool dns_eq = u_streq(have_lb, lb_dns, hostname);
+    // EnsureGlobalAcceleratorFor* (global_accelerator.go:112-211): the load balancer and its checks come from lbi_resolve
+    LbiRes res;
+    res.lb = GAR_NONE;
+    res.lb_dns = res.lb_arn = 0;
+    if (probe) res = W.lbi_res[jb + j];
+    const u32 lb = lbi_lb(res);
     bool go = false;
     if (probe) {
-      if (!have_lb) {
+      const u32 v = lbi_verdict(res);
+      if (v == LBI_NOT_FOUND) {
         result = GAR_STATUS(GAR_ST_ERR_RETRY, GAR_D_LB_NOT_FOUND, ev);
         stop = true;
-      } else if (!dns_eq) {
+      } else if (v == LBI_DNS_MISMATCH) {
         result = GAR_STATUS(GAR_ST_ERR_RETRY, GAR_D_LB_DNS_MISMATCH, ev);
         stop = true;
-      } else if (lb_state != GAR_LB_ACTIVE) {
+      } else if (v == LBI_NOT_ACTIVE) {
         result = GAR_STATUS(GAR_ST_REQUEUE_30S, 0, ev);
         stop = true;
       } else {
         go = true;
       }
     }
+    const Str lb_dns = mkstr(A.slab, res.lb_dns);
     // the first iteration that gets here evaluates the snapshot (all lanes together); later ones (rare) evaluate what the
     // object's own earlier ops left behind, scalar
     const bool later = go && prev_lb != GAR_NONE;
     if (later) ga_later_step(T, W, i, kind, okey, jb, j, lb, prev_lb, pending, s, &ev);
     go = go && !later;
     OwnRange oc = go ? own_accs(W, i) : OwnRange{0, 0};
-    Str lb_arn = go ? mkstr(A.slab, A.lb_arn[lb]) : Str{A.slab, 0};
+    Str lb_arn = go ? mkstr(A.slab, res.lb_arn) : Str{A.slab, 0};
     u32 nacc = 0;
     for (;;) {  // accelerators of the owner, in ListAccelerators order
       bool a = go && !stop && oc.pos < oc.end;
@@ -1063,7 +1079,10 @@ GAR_HD u32 ga_reconcile(const DevTables &T, const Work &W, u32 i, bool valid, Op
       d.flags = 0;
       if (a) d = W.acc_digest[acc];
       // updateGlobalAcceleratorFor{Service,Ingress} (:290-410)
-      if (u_accelerator_changed(T, W, a, i, dv, kind, acc, d, okey, lb_dns)) s.put(GAR_OP_HEAD(GAR_OP_GA_UPDATE_ACCEL, GAR_CTRL_GA, kind), i, j, acc, lb, GAR_NONE);
+      // the first accelerator lbi_resolve found by the hostname carries a target-hostname tag equal to the hostname, and so
+      // (verdict ok) to the load balancer's DNS name: the common case needs no byte compare here
+      const bool thost_eq = a && acc == lbi_acc(res);
+      if (u_accelerator_changed(T, W, a, i, dv, kind, acc, d, okey, lb_dns, thost_eq)) s.put(GAR_OP_HEAD(GAR_OP_GA_UPDATE_ACCEL, GAR_CTRL_GA, kind), i, j, acc, lb, GAR_NONE);
       u32 eg = GAR_NONE;
       if (a) {
         if (d.flags & ACCD_LIS_MANY) {
@@ -1144,9 +1163,8 @@ GAR_HD void ga_later_step(const DevTables &T, const Work &W, u32 i, u32 kind, St
     bool replaced = created;
     for (u32 jp = 0; jp < j && !replaced; jp++) {
       if (W.tok_code[jb + jp] > GAR_TOK_NLB) continue;  // DetectCloudProvider error: that iteration was skipped
-      u32 st;
-      u32 lbp = find_lb(T, W, mkstr(T.o.slab, W.tok_region[jb + jp]), mkstr(T.o.slab, W.tok_name[jb + jp]), &st);
-      if (lbp != GAR_NONE && !eg_contains(T, d, mkstr(A.slab, A.lb_arn[lbp]))) replaced = true;
+      const LbiRes rp = W.lbi_res[jb + jp];
+      if (lbi_lb(rp) != GAR_NONE && !eg_contains(T, d, mkstr(A.slab, rp.lb_arn))) replaced = true;
     }
     const bool contains = replaced ? !arn_differs : eg_contains(T, d, lb_arn);
     if (!contains) s.put(GAR_OP_HEAD(GAR_OP_GA_UPDATE_EG, GAR_CTRL_GA, kind), i, j, acc, created ? GAR_PENDING : d.eg, lb);
@@ -1311,7 +1329,6 @@ GAR_HD u32 r53_reconcile(const DevTables &T, const Work &W, u32 i, bool valid, O
     bool act = ensure && !stop && j < nj;
     if (!GAR_ANY(act)) break;
     bool probe = false;
-    Str lbhost{o.slab, 0};
     if (act) {
       u32 code = W.tok_code[jb + j];
       if (code == GAR_TOK_PANIC) {
@@ -1323,13 +1340,17 @@ GAR_HD u32 r53_reconcile(const DevTables &T, const Work &W, u32 i, bool valid, O
         stop = true;
       } else {
         probe = true;
-        lbhost = mkstr(o.slab, o.lbi_hostname[jb + j]);
       }
     }
-    // ensureRoute53 (route53.go:56-130)
-    u32 acc = GAR_NONE;
+    // ensureRoute53 (route53.go:56-130): the accelerators of the lbIngress hostname come from lbi_resolve
+    u32 acc = GAR_NONE, nacc = 0;
     gar_str acc_dns_ref = 0;
-    u32 nacc = u_find_by_hostname(T, W, probe, lbhost, &acc, &acc_dns_ref);
+    if (probe) {
+      const LbiRes res = W.lbi_res[jb + j];
+      nacc = lbi_acc_count(res);
+      acc = lbi_acc(res);
+      acc_dns_ref = res.acc_dns;
+    }
     bool go = false;
     if (probe) {
       if (nacc > 1) {
@@ -1427,7 +1448,8 @@ GAR_HD void r53_prepare(const DevTables &T, const Work &W, u32 i, u32 t, bool va
   const gar_objects &o = T.o;
   u32 mode = R53_MODE_DONE, st = GAR_STATUS(GAR_ST_IGNORED, 0, 0), npairs = 0;
   bool probe = false;
-  Str lbhost{o.slab, 0}, hostnames{o.slab, 0};
+  u32 lbi = 0;
+  Str hostnames{o.slab, 0};
   if (valid) {
     u32 dv = W.derived[i];
     if (dv & GAR_DV_R53_ELIGIBLE) {
@@ -1443,15 +1465,21 @@ GAR_HD void r53_prepare(const DevTables &T, const Work &W, u32 i, u32 t, bool va
         else if (code >= GAR_TOK_ERR_NOT_ELB) st = GAR_STATUS(GAR_ST_ERR_RETRY, GAR_D_NOT_ELB + (code - GAR_TOK_ERR_NOT_ELB), 0);
         else {
           probe = true;
-          lbhost = mkstr(o.slab, o.lbi_hostname[jb]);
+          lbi = jb;
           hostnames = mkstr(o.slab, W.ann_r53[i]);
         }
       }
     }
   }
-  u32 acc = GAR_NONE;
+  // the accelerators of the lbIngress hostname (ListGlobalAcceleratorByHostname) come from lbi_resolve
+  u32 acc = GAR_NONE, nacc = 0;
   gar_str acc_dns = 0;
-  u32 nacc = u_find_by_hostname(T, W, probe, lbhost, &acc, &acc_dns);
+  if (probe) {
+    const LbiRes res = W.lbi_res[lbi];
+    nacc = lbi_acc_count(res);
+    acc = lbi_acc(res);
+    acc_dns = res.acc_dns;
+  }
   bool go = false;
   if (probe) {
     if (nacc > 1) st = GAR_STATUS(GAR_ST_REQUEUE_60S, GAR_D_ACCEL_MANY, 0);
