@@ -34,7 +34,10 @@ typedef uint64_t u64;
 typedef int32_t i32;
 typedef int64_t i64;
 
-#define GAR_SLAB_PAD 32  // bytes of readable zero padding the engine keeps after every slab (wide loads may over-read)
+// Readable bytes behind every slab (wide loads may over-read).  No result depends on their values: the engine zeroes the pad
+// of the slabs it allocates, but an attached slab (gar_snapshot_attach_device) or a sharded sub-snapshot, whose slab is the
+// receive buffers themselves, may hold anything there.
+#define GAR_SLAB_PAD 32
 
 // ------------------------------------------------------------------ string views
 

@@ -694,7 +694,8 @@ int gar_bindings_diff(gar_engine *e, const gar_bindings *bindings, gar_changeset
        gar_shard_pack(e, send)                                send: device buffer of sum(send_bytes), blobs back to back
        exchange the blobs (all-to-all, sizes from gar_shard_blob_bytes(received meta row))
        gar_shard_unpack(e, round, recv, recv_meta)            recv: the received blobs back to back, in rank order, with
-                                                              32 readable bytes behind them.  The string bytes are NOT
+                                                              32 readable bytes behind them (their values, like those of
+                                                              the blobs' alignment gaps, do not matter).  The string bytes are NOT
                                                               copied: the sub-snapshot's strings live in BOTH rounds' receive
                                                               buffers, which must stay alive and unchanged until the last
                                                               diff of this exchange (the next gar_shard_route(.., 1) or
