@@ -185,6 +185,24 @@ class ZoneDeltaResult(ActualDeltaResult):
     FIELDS = ("n_zones", "n_records", "n_values", "slab_base", "slab_len")
 
 
+class GarRecordDelta(C.Structure):
+    _fields_ = [("rows", C.POINTER(GarActual)), ("zone_target", _u32p), ("rec_at", _u32p), ("n_deleted", C.c_uint32), ("deleted", _u32p)]
+
+
+class GarRecordDeltaResult(C.Structure):
+    _fields_ = [("n_records", C.c_uint32), ("n_values", C.c_uint32), ("slab_base", C.c_uint64), ("slab_len", C.c_uint64)]
+
+
+class RecordDeltaResult(ActualDeltaResult):
+    """Outcome of one record delta (include/garecon.h gar_record_delta_result): n_records, n_values, slab_base, slab_len."""
+    __slots__ = ()
+    FIELDS = ("n_records", "n_values", "slab_base", "slab_len")
+
+
+class GarRecordReadSet(C.Structure):
+    _fields_ = [("n_records", C.c_uint32), ("rec_rows", _u32p), ("opaque", C.c_void_p)]
+
+
 COMPACT_OBJECTS, COMPACT_ACTUAL = 1, 2
 
 
@@ -355,6 +373,10 @@ def load_library(path: os.PathLike | None = None) -> C.CDLL:
     lib.gar_read_set.restype = C.c_int
     lib.gar_read_set_free.argtypes = [C.c_void_p, C.POINTER(GarReadSet)]
     lib.gar_read_set_free.restype = None
+    lib.gar_read_records.argtypes = [C.c_void_p, C.POINTER(GarKeyset), C.POINTER(GarRecordReadSet)]
+    lib.gar_read_records.restype = C.c_int
+    lib.gar_read_records_free.argtypes = [C.c_void_p, C.POINTER(GarRecordReadSet)]
+    lib.gar_read_records_free.restype = None
     lib.gar_bindings_diff.argtypes = [C.c_void_p, C.POINTER(GarBindings), C.POINTER(GarChangeset)]
     lib.gar_bindings_diff.restype = C.c_int
     lib.gar_snapshot_apply_objects.argtypes = [C.c_void_p, C.POINTER(GarObjectDelta), C.POINTER(GarDeltaResult)]
@@ -363,6 +385,8 @@ def load_library(path: os.PathLike | None = None) -> C.CDLL:
     lib.gar_snapshot_apply_actual.restype = C.c_int
     lib.gar_snapshot_apply_zones.argtypes = [C.c_void_p, C.POINTER(GarZoneDelta), C.POINTER(GarZoneDeltaResult)]
     lib.gar_snapshot_apply_zones.restype = C.c_int
+    lib.gar_snapshot_apply_records.argtypes = [C.c_void_p, C.POINTER(GarRecordDelta), C.POINTER(GarRecordDeltaResult)]
+    lib.gar_snapshot_apply_records.restype = C.c_int
     lib.gar_snapshot_compact.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(GarCompactResult)]
     lib.gar_snapshot_compact.restype = C.c_int
     lib.gar_snapshot_export.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.POINTER(GarObjects), C.c_void_p, C.c_uint64,
@@ -403,7 +427,7 @@ def load_library(path: os.PathLike | None = None) -> C.CDLL:
 
 EXPORTED_SYMBOLS = (
     "gar_engine_create", "gar_engine_destroy", "gar_snapshot_load", "gar_snapshot_attach_device", "gar_diff",
-    "gar_diff_device", "gar_diff_keys", "gar_read_set", "gar_read_set_free", "gar_bindings_diff", "gar_snapshot_apply_objects", "gar_snapshot_apply_actual", "gar_snapshot_apply_zones", "gar_snapshot_compact", "gar_snapshot_export", "gar_snapshot_read_slab", "gar_shard_route", "gar_shard_pack", "gar_shard_unpack", "gar_shard_blob_bytes",
+    "gar_diff_device", "gar_diff_keys", "gar_read_set", "gar_read_set_free", "gar_bindings_diff", "gar_snapshot_apply_objects", "gar_snapshot_apply_actual", "gar_snapshot_apply_zones", "gar_snapshot_apply_records", "gar_read_records", "gar_read_records_free", "gar_snapshot_compact", "gar_snapshot_export", "gar_snapshot_read_slab", "gar_shard_route", "gar_shard_pack", "gar_shard_unpack", "gar_shard_blob_bytes",
     "gar_shard_arena", "gar_shard_open_peers", "gar_shard_pack_peers",
     "gar_changeset_free", "gar_last_error", "gar_version", "gar_algorithmic_bytes",
     "gar_last_stage_timings", "gar_last_counters",
@@ -514,6 +538,30 @@ class Engine:
         res = GarZoneDeltaResult()
         self._check(self.lib.gar_snapshot_apply_zones(self._h, C.byref(d), C.byref(res)))
         return ZoneDeltaResult(res)
+
+    def apply_records(self, rows: GarActual | None = None, zone_target=(), rec_at=(), deleted=()) -> RecordDeltaResult:
+        """Record delta against the loaded snapshot (include/garecon.h gar_snapshot_apply_records).  `rows`: a GarActual holding
+        re-described record sets grouped by zone, e.g. tables.pack([], {"zones": [...]}).actual (its buffers must stay alive for
+        the call); zone_target[k]: the resident zone of delta zone k (strictly ascending); rec_at[k]: the resident record row
+        delta record k is listed in front of (non-decreasing); `deleted`: resident record rows removed with their values."""
+        zt, ra, dl = (np.ascontiguousarray(np.asarray(list(v), dtype=np.uint32).reshape(-1)) for v in (zone_target, rec_at, deleted))
+        p = lambda a: a.ctypes.data_as(_u32p)  # noqa: E731  (the arrays stay alive until the call returns)
+        d = GarRecordDelta(C.pointer(rows) if rows is not None else None, p(zt), p(ra), len(dl), p(dl))
+        res = GarRecordDeltaResult()
+        self._check(self.lib.gar_snapshot_apply_records(self._h, C.byref(d), C.byref(res)))
+        return RecordDeltaResult(res)
+
+    def read_records(self, rows, deleted=()) -> np.ndarray:
+        """The resident record rows the Route53 decisions of this keyset read (include/garecon.h gar_read_records), ascending:
+        what a worker re-describes and applies with apply_records before diff_keys(rows, deleted)."""
+        ks = make_keyset(rows, deleted)
+        rs = GarRecordReadSet()
+        self._check(self.lib.gar_read_records(self._h, C.byref(ks), C.byref(rs)))
+        try:
+            out = _np_from(rs.rec_rows, rs.n_records, np.uint32)
+        finally:
+            self.lib.gar_read_records_free(self._h, C.byref(rs))
+        return out
 
     def compact(self, groups: int = COMPACT_OBJECTS | COMPACT_ACTUAL) -> GarCompactResult:
         """Rebuild the resident slabs of `groups` (COMPACT_OBJECTS | COMPACT_ACTUAL) dense on the device (include/garecon.h

@@ -290,6 +290,35 @@ struct FDeltaZoneMap {
     }
   }
 };
+// record deltas (include/garecon.h "record deltas") run FDeltaZoneMap over the record table (del: deleted record rows, at: rec_at)
+// and re-lay record -> value; the zone table keeps its rows and gets new begins from these counts + one scan.  Zone z's new count:
+// its resident records, minus the deleted ones inside its range, plus the records of the delta zone that targets it (target
+// strictly ascending, ub: the delta's zone_rec_begin).  Zone row n: the 0 that becomes the scan's total
+struct FDeltaRecZoneCounts {
+  const u32 *rb, *del, *target, *ub;
+  u32 nd, nt, n;
+  u32 *db;
+  GAR_HD void operator()(u32 z) const {
+    if (z == n) {
+      db[n] = 0;
+      return;
+    }
+    u32 c = rb[z + 1] - rb[z] - (delta_rank(del, nd, rb[z + 1]) - delta_rank(del, nd, rb[z]));
+    const u32 k = delta_rank(target, nt, z);
+    if (k < nt && target[k] == z) c += ub[k + 1] - ub[k];
+    db[z] = c;
+  }
+};
+// the records of delta zone k must be placed inside its resident zone: rec_at within [rb[z], rb[z + 1]] for z = target[k] (rec_at
+// is non-decreasing, checked on the host, so the first and the last record of the zone decide)
+struct FDeltaRecAt {
+  const u32 *rb, *target, *ub, *at;
+  u32 *bad;
+  GAR_HD void operator()(u32 k) const {
+    const u32 k0 = ub[k], k1 = ub[k + 1], z = target[k];
+    if (k0 < k1 && (at[k0] < rb[z] || at[k1 - 1] > rb[z + 1])) *bad = 1;
+  }
+};
 
 // column layout of gar_actual: table, element width, gar_str or not, and the child table of a begin column (AT_N: none)
 struct ActualColInfo {
@@ -736,6 +765,74 @@ struct ActualSplicer {
     return GAR_OK;
   }
 
+  // the record splice of include/garecon.h "record deltas": the host checks the delta's own order (O(delta)), two small kernels
+  // check its zones against the resident ones, FDeltaZoneMap writes the record table's source map, FDeltaRecZoneCounts + a scan
+  // give zone_rec_begin, and relayout() re-lays record -> value.  GAR_OK, GAR_E_INVALID (error says why; nothing changed) or
+  // another gar_rc
+  int apply(const gar_record_delta &d, gar_record_delta_result &out) {
+    const gar_actual no_rows = empty_table();
+    const gar_actual &H = d.rows ? *d.rows : no_rows;
+    R = T.a;
+    if (H.n_lbs || H.n_accels || H.n_tags || H.n_listeners || H.n_port_ranges || H.n_egs || H.n_endpoints)
+      return invalid("rows: a record delta carries zones with their record sets only, no load balancer or accelerator rows");
+    error = delta_check_actual(H);
+    if (!error.empty()) return GAR_E_INVALID;
+    const u32 n = R.n_records, nz = H.n_zones, ni = H.n_records, nd = d.n_deleted;
+    if ((nz && !d.zone_target) || (ni && !d.rec_at) || (nd && !d.deleted)) return invalid("NULL zone_target, rec_at or deleted array");
+    for (u32 k = 0; k < nz; k++) {
+      if (d.zone_target[k] >= R.n_zones) return invalid("zone_target out of range (adding hosted zones is gar_snapshot_apply_zones)");
+      if (k && d.zone_target[k] <= d.zone_target[k - 1]) return invalid("zone_target is not strictly ascending");
+    }
+    for (u32 k = 0; k < ni; k++) {
+      if (d.rec_at[k] > n) return invalid("rec_at out of range");
+      if (k && d.rec_at[k] < d.rec_at[k - 1]) return invalid("rec_at decreases");
+    }
+    std::vector<u32> del(d.deleted, d.deleted + nd);
+    std::sort(del.begin(), del.end());
+    for (u32 m = 0; m < nd; m++) {
+      if (del[m] >= n) return invalid("deleted record row out of range");
+      if (m && del[m] == del[m - 1]) return invalid("a record row appears twice in deleted");
+    }
+    if ((u64)n - nd + ni >= (1u << 27)) return invalid("too many records for one snapshot");
+    const u32 n_new = n - nd + ni;
+    base = ni ? (R.slab_len + 15) & ~(u64)15 : 0;
+    if (ni && base + H.slab_len + GAR_SLAB_PAD >= (1ull << GAR_STR_OFF_BITS)) return invalid("the resident AWS slab would outgrow 2^40 bytes");
+    const u32 *target = nullptr, *at = nullptr;
+    if (nz) {
+      const u32 zero[2] = {0, 0};
+      u32 *bad = (u32 *)up(DS_A_FLAG, zero, 8);
+      target = zone_names_launch(H, d.zone_target, bad);
+      const u32 *ub = (const u32 *)up(DS_A_UP + AC_ZONE_REC_B, H.zone_rec_begin, 4 * (size_t)(nz + 1));
+      at = (const u32 *)up(DS_A_PAIRS + AT_REC, d.rec_at, 4 * (size_t)ni);
+      be.for_each("delta_record_at", nz, FDeltaRecAt{R.zone_rec_begin, target, ub, at, bad + 1});
+      u32 flag[2];
+      be.download(flag, bad, 8);
+      if (flag[0]) return invalid("a delta zone's zone_name differs from the name of the resident zone it targets");
+      if (flag[1]) return invalid("rec_at outside the record range of its zone");
+    }
+    N = R;
+    if (ni || nd) {
+      stage(H, ni != 0);
+      const u32 *ddel = (const u32 *)up(DS_A_DEL + AT_REC, del.data(), 4 * (size_t)nd);
+      u32 *src = (u32 *)be.delta_scratch(DS_A_SRC + AT_REC, 4 * (size_t)(n_new + 1));
+      if (n + ni) be.for_each("delta_record_map", n + ni, FDeltaZoneMap{ddel, at, nd, ni, n, src});
+      const u32 nzones = R.n_zones;
+      u32 *zb = (u32 *)standby(AC_ZONE_REC_B, 4 * (size_t)(nzones + 1));
+      be.for_each("delta_record_zone_counts", nzones + 1, FDeltaRecZoneCounts{R.zone_rec_begin, ddel, target, U.zone_rec_begin, nd, nz, nzones, zb});
+      be.exclusive_scan(zb, nzones + 1);
+      const int rc = relayout(AT_REC, src, n_new);
+      if (rc != GAR_OK) return rc;
+      for (int c = 0; c < AC_N; c++)
+        if (written[c]) be.delta_actual_swap(c);
+      T.a = N;
+    }
+    out.n_records = T.a.n_records;
+    out.n_values = T.a.n_values;
+    out.slab_base = base;
+    out.slab_len = T.a.slab_len;
+    return GAR_OK;
+  }
+
  private:
   int invalid(const std::string &msg) {
     error = msg;
@@ -809,6 +906,15 @@ struct ActualSplicer {
   }
 
   bool zone_names_match(const gar_actual &H, const u32 *target) {
+    const u32 zero = 0;
+    u32 *bad = (u32 *)up(DS_A_FLAG, &zero, 4);
+    zone_names_launch(H, target, bad);
+    u32 flag = 0;
+    be.download(&flag, bad, 4);
+    return flag == 0;
+  }
+  // queues the zone-name check (delta zone k against resident zone target[k]; *bad = 1 on a mismatch) -> target on the device
+  const u32 *zone_names_launch(const gar_actual &H, const u32 *target, u32 *bad) {
     std::vector<u8> zslab;
     std::vector<gar_str> zref(H.n_zones);
     for (u32 k = 0; k < H.n_zones; k++) {
@@ -818,14 +924,11 @@ struct ActualSplicer {
       zslab.insert(zslab.end(), p, p + len);
     }
     zslab.resize(zslab.size() + GAR_SLAB_PAD, 0);
-    const u32 zero = 0;
-    u32 *bad = (u32 *)up(DS_A_FLAG, &zero, 4);
+    const u32 *dtarget = (const u32 *)up(DS_A_ZTARGET, target, 4 * (size_t)H.n_zones);
     be.for_each("delta_zone_names", H.n_zones,
-                FDeltaZoneName{R.slab, R.zone_name, (const u32 *)up(DS_A_ZTARGET, target, 4 * (size_t)H.n_zones), (const u8 *)up(DS_A_ZSLAB, zslab.data(), zslab.size()),
+                FDeltaZoneName{R.slab, R.zone_name, dtarget, (const u8 *)up(DS_A_ZSLAB, zslab.data(), zslab.size()),
                                (const gar_str *)up(DS_A_ZREF, zref.data(), 8 * (size_t)H.n_zones), bad});
-    u32 flag = 0;
-    be.download(&flag, bad, 4);
-    return flag == 0;
+    return dtarget;
   }
 
   // source map of a root table: identity or the survivors of the deletes, then the replaced / appended rows

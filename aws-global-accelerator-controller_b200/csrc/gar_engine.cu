@@ -1388,7 +1388,7 @@ static void do_apply(gar_engine *e, const gar_object_delta *d, gar_delta_result 
   }
 }
 
-// AWS deltas and zone deltas (gar_actual_delta / gar_zone_delta): the same splicer, state checks and prepared-state drop
+// AWS, zone and record deltas (gar_actual_delta / gar_zone_delta / gar_record_delta): the same splicer, state checks and prepared-state drop
 template <class Delta, class Result>
 static void do_apply_actual(gar_engine *e, const Delta *d, Result *out) {
   if (!e->loaded) throw StateError{"no snapshot loaded"};
@@ -1537,8 +1537,8 @@ static void upload_keyset(gar_engine *e, const gar_keyset *ks, const u32 **rows_
   *D = DelKeys{dkind, dkey, dslab};
 }
 
-static void do_read_set(gar_engine *e, const gar_keyset *ks, gar_readset *out) {
-  memset(out, 0, sizeof(*out));
+// gar_read_set and gar_read_records: the checks, the keyset upload and the ReadSetter run (records: the record read set)
+static ReadSetter<gar_engine, Pipeline<gar_engine>> run_read_setter(gar_engine *e, const gar_keyset *ks, bool records) {
   if (!e->loaded) throw StateError{"no snapshot loaded"};
   if (e->shard_home || e->shard_round != 0) throw StateError{"the read set is not available in sharded mode"};
   check_keyset(e, ks);
@@ -1555,16 +1555,23 @@ static void do_read_set(gar_engine *e, const gar_keyset *ks, gar_readset *out) {
   P.allow_empty_cache = e->allow_empty_cache;
   if (e->reprepare) P.prepared = false;
   ReadSetter<gar_engine, Pipeline<gar_engine>> R{*e, P, e->rs_clean};
+  R.records = records;
   const int rc = R.run(rows, ks->n_rows, D, ks->n_deleted);
   if (rc == GAR_E_INVALID) throw InvalidError{"objects layout rule violated: obj_ns and obj_name must be slices of one \"ns/name\" key string"};
   if (rc != GAR_OK) throw InvalidError{"the snapshot did not settle: an intermediate relation kept outgrowing its buffer"};
-  HostReadSet *h;
-  if (!e->free_read_sets.empty()) {
-    h = e->free_read_sets.back();
-    e->free_read_sets.pop_back();
-  } else {
-    h = new HostReadSet();
-  }
+  return R;
+}
+static HostReadSet *host_read_set(gar_engine *e) {
+  if (e->free_read_sets.empty()) return new HostReadSet();
+  HostReadSet *h = e->free_read_sets.back();
+  e->free_read_sets.pop_back();
+  return h;
+}
+
+static void do_read_set(gar_engine *e, const gar_keyset *ks, gar_readset *out) {
+  memset(out, 0, sizeof(*out));
+  ReadSetter<gar_engine, Pipeline<gar_engine>> R = run_read_setter(e, ks, false);
+  HostReadSet *h = host_read_set(e);
   out->opaque = h;
   const u32 nl = R.n[RS_LB], na = R.n[RS_ACC], nz = R.n[RS_ZONE], nm = R.n[RS_MISS];
   u32 *hr = (u32 *)e->pin_ensure(h->rows, 4 * ((size_t)nl + na + nz + 2 * (size_t)nm));
@@ -1592,6 +1599,20 @@ static void do_read_set(gar_engine *e, const gar_keyset *ks, gar_readset *out) {
   out->lb_miss_j = hr + nl + na + nz + nm;
   out->lb_miss_name = hs;
   out->lb_miss_region = hs + nm;
+}
+
+static void do_read_records(gar_engine *e, const gar_keyset *ks, gar_record_readset *out) {
+  memset(out, 0, sizeof(*out));
+  ReadSetter<gar_engine, Pipeline<gar_engine>> R = run_read_setter(e, ks, true);
+  HostReadSet *h = host_read_set(e);
+  out->opaque = h;  // the same pool as gar_read_set's: only `rows` is used
+  const u32 nr = R.n[RS_REC];
+  u32 *hr = (u32 *)e->pin_ensure(h->rows, 4 * (size_t)nr);
+  if (nr) CK(cudaMemcpyAsync(hr, R.out.rows[RS_REC], 4 * (size_t)nr, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  CK(cudaGetLastError());
+  out->n_records = nr;
+  out->rec_rows = hr;
 }
 
 static void do_diff(gar_engine *e, gar_changeset *out, bool to_host, const gar_keyset *ks = nullptr, const gar_bindings *bd = nullptr) {
@@ -1944,6 +1965,18 @@ void gar_read_set_free(gar_engine *e, gar_readset *rs) {
   memset(rs, 0, sizeof(*rs));
 }
 
+int gar_read_records(gar_engine *e, const gar_keyset *keys, gar_record_readset *out) {
+  if (!out || !keys) return GAR_E_INVALID;
+  return guarded(e, [&] { do_read_records(e, keys, out); });
+}
+
+void gar_read_records_free(gar_engine *e, gar_record_readset *rs) {
+  if (!e || !rs) return;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (rs->opaque) e->free_read_sets.push_back((HostReadSet *)rs->opaque);
+  memset(rs, 0, sizeof(*rs));
+}
+
 int gar_bindings_diff(gar_engine *e, const gar_bindings *bindings, gar_changeset *out) {
   if (!out || !bindings) return GAR_E_INVALID;
   return guarded(e, [&] { do_diff(e, out, true, nullptr, bindings); });
@@ -1960,6 +1993,11 @@ int gar_snapshot_apply_actual(gar_engine *e, const gar_actual_delta *d, gar_actu
 }
 
 int gar_snapshot_apply_zones(gar_engine *e, const gar_zone_delta *d, gar_zone_delta_result *out) {
+  if (!d || !out) return GAR_E_INVALID;
+  return guarded(e, [&] { do_apply_actual(e, d, out); });
+}
+
+int gar_snapshot_apply_records(gar_engine *e, const gar_record_delta *d, gar_record_delta_result *out) {
   if (!d || !out) return GAR_E_INVALID;
   return guarded(e, [&] { do_apply_actual(e, d, out); });
 }

@@ -1452,6 +1452,7 @@ struct Pipeline {
 //
 // Backend: for_each, fill32, exclusive_scan(u64 *), download, and read_set_buf(k, bytes) — scratch that no recorded launch
 // sequence holds, so the call grows it without dropping the full diff's graph (the 64-bit scan keeps its own tile states too).
+// The record read set (gar_read_records) is the same run with `records` set: other items, one bitmap over record rows.
 // Steps: prepare as gar_diff_keys does (Pipeline::run_with) -> items per key, scan -> mark (one thread per item) -> popcount
 // per bitmap word, scan -> emit rows ascending, zeroing every word read: the bitmaps are all zero between calls, so a call
 // costs O(keys + items + table rows / 32).  After a failed call they are cleared again before they are trusted.
@@ -1470,8 +1471,10 @@ struct FReadSetCount {
   DelKeys D;
   Cursor *cur;  // [2 nd]
   u64 *items;   // [m + nd + 1]
+  bool recs;    // the record read set (gar_read_records)
   GAR_HD void operator()(u32 t) const {
-    if (t < m) items[t] = read_set_row_items(T, W, rows[t]);
+    if (t < m) items[t] = recs ? read_records_row_items(W, rows[t]) : read_set_row_items(T, W, rows[t]);
+    else if (recs) items[t] = read_records_deleted_items(W, D.kind[t - m], mkstr(D.slab, D.key[t - m]), cur + 2 * (t - m));
     else items[t] = read_set_deleted_items(W, D.kind[t - m], mkstr(D.slab, D.key[t - m]), cur + 2 * (t - m));
   }
 };
@@ -1485,6 +1488,7 @@ struct FReadSetMark {
   const u64 *items;  // exclusive-scanned
   u64 base;
   ReadSetBits B;
+  bool recs;
   GAR_HD void operator()(u32 x) const {
     const u64 q = base + x;
     u32 lo = 0, hi = nkeys;  // the last key whose first item is <= q (a key with no items shares its offset with the next)
@@ -1494,8 +1498,14 @@ struct FReadSetMark {
       else hi = mid;
     }
     const u32 r = (u32)(q - items[lo]);
-    if (lo < m) read_set_row_item(T, W, B, rows[lo], r);
-    else read_set_deleted_item(T, W, B, D.kind[lo - m], mkstr(D.slab, D.key[lo - m]), cur + 2 * (lo - m), r);
+    if (lo < m) {
+      if (recs) read_records_row_item(T, W, B, rows[lo], r);
+      else read_set_row_item(T, W, B, rows[lo], r);
+    } else if (recs) {
+      read_records_deleted_item(T, W, B, D.kind[lo - m], mkstr(D.slab, D.key[lo - m]), cur + 2 * (lo - m), r);
+    } else {
+      read_set_deleted_item(T, W, B, D.kind[lo - m], mkstr(D.slab, D.key[lo - m]), cur + 2 * (lo - m), r);
+    }
   }
 };
 struct FReadSetPopc {
@@ -1557,6 +1567,7 @@ struct ReadSetter {
   Be &be;
   Pipe &P;
   ReadSetClean &clean;
+  bool records = false;  // gar_read_records: only the record bitmap (RS_REC) is sized and filled
   enum { RB_ITEMS, RB_CUR, RB_BITS, RB_CNT, RB_SIZES, RB_OUT32, RB_OUT64, RB_N };
   // rows of each bitmap (RS_N) and the size of each, device pointers valid until the next call
   ReadSetOut out;
@@ -1573,7 +1584,8 @@ struct ReadSetter {
     const u32 nk = m + nd;
     u64 *items = (u64 *)be.read_set_buf(RB_ITEMS, 8 * ((size_t)nk + 2));
     Cursor *cur = (Cursor *)be.read_set_buf(RB_CUR, sizeof(Cursor) * (2 * (size_t)nd + 1));
-    const u32 size[RS_N] = {T.a.n_lbs, T.a.n_accels, T.a.n_zones, T.o.n_lbi};
+    const u32 size[RS_N] = {records ? 0 : T.a.n_lbs, records ? 0 : T.a.n_accels, records ? 0 : T.a.n_zones, records ? 0 : T.o.n_lbi,
+                            records ? T.a.n_records : 0};
     ReadSetBits B;
     B.wb[0] = 0;
     for (int s = 0; s < RS_N; s++) B.wb[s + 1] = B.wb[s] + (size[s] + 31) / 32;
@@ -1583,14 +1595,14 @@ struct ReadSetter {
     clean.bits = B.bits;
     clean.words = 0;
 
-    if (nk) be.for_each("read_set_count", nk, FReadSetCount{T, W, rows, m, D, cur, items});
+    if (nk) be.for_each("read_set_count", nk, FReadSetCount{T, W, rows, m, D, cur, items, records});
     be.fill32((u32 *)(items + nk), 0, 2);
     be.exclusive_scan(items, nk + 1);
     u64 total = 0;
     be.download(&total, items + nk, 8);
     constexpr u64 CHUNK = 1ull << 30;
     for (u64 b = 0; b < total; b += CHUNK)
-      be.for_each("read_set_mark", (u32)(total - b < CHUNK ? total - b : CHUNK), FReadSetMark{T, W, rows, m, nk, D, cur, items, b, B});
+      be.for_each("read_set_mark", (u32)(total - b < CHUNK ? total - b : CHUNK), FReadSetMark{T, W, rows, m, nk, D, cur, items, b, B, records});
 
     u64 *cnt = (u64 *)be.read_set_buf(RB_CNT, 8 * ((size_t)nw + 2));
     u64 *sizes = (u64 *)be.read_set_buf(RB_SIZES, 8 * (RS_N + 1));
@@ -1598,7 +1610,7 @@ struct ReadSetter {
     be.fill32((u32 *)(cnt + nw), 0, 2);
     be.exclusive_scan(cnt, nw + 1);
     be.for_each("read_set_sizes", RS_N + 1, FReadSetSizes{cnt, B, sizes});
-    u32 *o32 = (u32 *)be.read_set_buf(RB_OUT32, 4 * ((size_t)size[0] + size[1] + size[2] + 2 * (size_t)size[3] + 1));
+    u32 *o32 = (u32 *)be.read_set_buf(RB_OUT32, 4 * ((size_t)size[0] + size[1] + size[2] + 2 * (size_t)size[3] + size[4] + 1));
     gar_str *o64 = (gar_str *)be.read_set_buf(RB_OUT64, 8 * (2 * (size_t)size[3] + 1));
     out.rows[RS_LB] = o32;
     out.rows[RS_ACC] = o32 + size[0];
@@ -1606,6 +1618,7 @@ struct ReadSetter {
     out.rows[RS_MISS] = nullptr;
     out.miss_obj = out.rows[RS_ZONE] + size[2];
     out.miss_j = out.miss_obj + size[3];
+    out.rows[RS_REC] = out.miss_j + size[3];
     out.miss_name = o64;
     out.miss_region = o64 + size[3];
     if (nw) be.for_each("read_set_emit", nw, FReadSetEmit{T, W, cnt, B, out});

@@ -1907,7 +1907,9 @@ GAR_HD u32 egb_reconcile(const DevTables &T, const Work &W, const DevBindings &B
 //                  segment, one for the pieces of its route53-hostname annotation;
 //   deleted key    one item per entry of its ix_owner bucket, one per entry of its ix_val bucket (the walks FDelKeyGa and
 //                  FDelKeyR53 make; a tag and key compare per entry decides).
-enum { RS_LB = 0, RS_ACC = 1, RS_ZONE = 2, RS_MISS = 3, RS_N = 4 };
+// The record read set (gar_read_records) is a fifth bitmap, over record rows, filled by the items of read_records_* below; each
+// call sizes only the bitmaps it fills, so the other call's bitmaps are empty.
+enum { RS_LB = 0, RS_ACC = 1, RS_ZONE = 2, RS_MISS = 3, RS_REC = 4, RS_N = 5 };
 struct ReadSetBits {
   u32 *bits;
   u32 wb[RS_N + 1];  // first word of each bitmap; wb[RS_N] = the total
@@ -1972,4 +1974,32 @@ GAR_HD void read_set_deleted_item(const DevTables &T, const Work &W, const ReadS
   }
   const IdxEntry e = load_entry(W.ix_val.ent + c[1].pos + (q - no));
   if (e.tag == c[1].tag && owned_match(T, e, kind, key)) rs_mark(B, RS_ZONE, owned_hit(e).zone);
+}
+
+// record read set: one item per owner value (an entry of the row's owned-value segment, or of the deleted key's ix_val bucket).
+// An item marks the record that carries the value and every alias record of the zone under that record's name (the ix_alias
+// walk of next_alias_any), so a hot TXT set's 10^5 values are 10^5 items.
+GAR_HD void read_records_mark(const DevTables &T, const Work &W, const ReadSetBits &B, const OwnedHit &h) {
+  rs_mark(B, RS_REC, h.rec);
+  const Str name = mkstr(T.a.slab, h.name);
+  Cursor c = idx_open(W.ix_alias, key_hash_zoned(h.zone, name));
+  IdxEntry e;
+  while (idx_next(W.ix_alias, c, &e))
+    if (e.a0 == h.zone && streq(mkstr(T.a.slab, e.s0), name)) rs_mark(B, RS_REC, e.row);
+}
+GAR_HD u32 read_records_row_items(const Work &W, u32 i) {
+  const OwnRange v = own_vals(W, i);
+  return v.end - v.pos;
+}
+GAR_HD void read_records_row_item(const DevTables &T, const Work &W, const ReadSetBits &B, u32 i, u32 q) {
+  read_records_mark(T, W, B, owned_hit(load_entry(W.own + own_vals(W, i).pos + q)));
+}
+// a deleted key's ix_val bucket, in c[0]
+GAR_HD u32 read_records_deleted_items(const Work &W, u32 kind, Str key, Cursor *c) {
+  c[0] = idx_open(W.ix_val, key_hash_kinded(kind, key));
+  return c[0].end - c[0].pos;
+}
+GAR_HD void read_records_deleted_item(const DevTables &T, const Work &W, const ReadSetBits &B, u32 kind, Str key, const Cursor *c, u32 q) {
+  const IdxEntry e = load_entry(W.ix_val.ent + c[0].pos + q);
+  if (e.tag == c[0].tag && owned_match(T, e, kind, key)) read_records_mark(T, W, B, owned_hit(e));
 }

@@ -361,6 +361,43 @@ class ActualMirror:
         s = self.sizes()
         return {"n_zones": s["n_zones"], "n_records": s["n_records"], "n_values": s["n_values"], "slab_base": base, "slab_len": self.slab_len}
 
+    def apply_records(self, rows: dict | None = None, zone_target=(), rec_at=(), deleted=()) -> dict:
+        """The rule of include/garecon.h "record deltas": inside each zone, the delta records placed in front of resident record
+        r (rec_at == r) come before r, in delta order, then r unless it is deleted; the ones placed behind the zone's last record
+        come last.  Values follow their records; zones, load balancers and accelerators keep their rows.  rows: an actual column
+        dict of zones with their records (own slab; zone k stands for resident zone zone_target[k]), or None.  -> the result of
+        the delta: n_records, n_values, slab_base, slab_len."""
+        cur = self.cur
+        zb = np.asarray(cur["zone_rec_begin"]).astype(np.int64)
+        n_rec = int(zb[-1])
+        at = np.asarray(rec_at, dtype=np.int64).reshape(-1)
+        zt = np.asarray(zone_target, dtype=np.int64).reshape(-1)
+        gone = np.zeros(n_rec, dtype=bool)
+        gone[np.asarray(deleted, dtype=np.int64).reshape(-1)] = True
+        base, both = 0, cur
+        if len(at):
+            padded = _pad16(cur)
+            base = len(padded["slab"])
+            both = tables.concat_cols(tables.ACT_TABLES, ["rec", "val"], [padded, rows])
+        # one sort key per placed record: (zone, position, inserts before the resident record at the same position, delta order)
+        res = np.flatnonzero(~gone)
+        res_zone = np.searchsorted(zb, res, side="right") - 1
+        ub = np.asarray(rows["zone_rec_begin"]).astype(np.int64) if len(at) else np.zeros(1, dtype=np.int64)
+        ins_zone = np.repeat(zt[:len(ub) - 1], ub[1:] - ub[:-1]) if len(at) else np.zeros(0, dtype=np.int64)
+        zone = np.concatenate([res_zone, ins_zone])
+        pos = np.concatenate([res, at])
+        tie = np.concatenate([np.ones(len(res), dtype=np.int64), np.zeros(len(at), dtype=np.int64)])
+        src = np.concatenate([res, n_rec + np.arange(len(at), dtype=np.int64)])
+        order = np.lexsort((src, tie, pos, zone))
+        new = {c: v for c, v in cur.items() if c != "slab"}
+        new["zone_rec_begin"] = np.concatenate([[0], np.cumsum(np.bincount(zone, minlength=len(zb) - 1))]).astype(np.uint32)
+        take_tree(both, "rec", src[order], new)
+        new["slab"] = np.asarray(both["slab"])
+        self.cur = new
+        self.slab_len = len(new["slab"])
+        s = self.sizes()
+        return {"n_records": s["n_records"], "n_values": s["n_values"], "slab_base": base, "slab_len": self.slab_len}
+
     def compact(self) -> int:
         """The mirror of gar_snapshot_compact(GAR_COMPACT_ACTUAL): the slab holds exactly the live strings.  -> slab_len."""
         self.cur = compact_actual(self.cur)
@@ -500,3 +537,139 @@ def objects_struct(cols: dict):
     empty_actual["slab"] = np.zeros(0, dtype=np.uint8)
     snap = tables.from_columns(cols, empty_actual)
     return snap, snap.objects
+
+
+# ------------------------------------------------------------------ record deltas (gar_snapshot_apply_records)
+
+def record_rows(cols: dict, zones, placed) -> dict:
+    """The `rows` of a record delta: zones `zones` (ascending resident zone rows of `cols`) with, per zone, the records `placed[k]`
+    (record rows of `cols`, in delta order), as a compact actual column dict with its own slab."""
+    rows = actual_rows(cols)
+    rows["zone_name"] = np.asarray(cols["zone_name"], dtype=np.uint64)[np.asarray(zones, dtype=np.int64)]
+    rec = np.asarray([r for rs in placed for r in rs], dtype=np.int64)
+    rows.update(take_tree(cols, "rec", rec))
+    rows["zone_rec_begin"] = np.concatenate([[0], np.cumsum([len(rs) for rs in placed])]).astype(np.uint32)
+    return compact_actual(rows)
+
+
+def record_churn(mirror: ActualMirror, rng: np.random.Generator, n_zones: int = 8, per_zone: int = 3):
+    """One batch of record-set edits inside resident zones, as a worker re-describes them: in `n_zones` random zones (and in the
+    first run of adjacent empty zones, when there is one) record sets replaced in place (alias target or values taken from
+    another record of the table), inserted at the zone's front, at its end and in between (copies of records from anywhere), and
+    deleted; now and then every record of a zone deleted.  -> keyword arguments of Engine.apply_records /
+    ActualMirror.apply_records, with rows = a compact actual column dict."""
+    cur = mirror.cur
+    zb = np.asarray(cur["zone_rec_begin"]).astype(np.int64)
+    nz, n_rec = len(zb) - 1, int(zb[-1])
+    if not nz:
+        return dict(rows=None, zone_target=np.zeros(0, dtype=np.uint32), rec_at=np.zeros(0, dtype=np.uint32), deleted=np.zeros(0, dtype=np.uint32))
+    zones = set(rng.choice(nz, size=min(nz, n_zones), replace=False).tolist())
+    empty = np.flatnonzero(zb[1:] == zb[:-1])
+    adj = empty[np.flatnonzero(empty[1:] == empty[:-1] + 1)] if len(empty) > 1 else empty[:0]
+    if len(adj):
+        zones.update([int(adj[0]), int(adj[0]) + 1])
+    elif len(empty):
+        zones.add(int(empty[0]))
+    alias = np.flatnonzero(np.asarray(cur["rec_has_alias"]) != 0)
+    extra = {}  # delta record -> (column, value) overrides, applied after the records are taken
+    targets, placed, at, deleted = [], [], [], []
+    for z in sorted(zones):
+        a, b = int(zb[z]), int(zb[z + 1])
+        ins = []  # (rec_at, source record row, override or None)
+        if b > a and rng.random() < 0.1:
+            deleted.extend(range(a, b))  # the zone's every record set deleted ...
+            if rng.random() < 0.5 and n_rec:
+                ins.append((b, int(rng.integers(0, n_rec)), None))  # ... and one listed again behind them
+        else:
+            for r in (rng.choice(np.arange(a, b), size=min(b - a, per_zone), replace=False).tolist() if b > a else []):
+                c = rng.random()
+                if c < 0.4:  # replaced: the same set with another alias target or another record's values
+                    deleted.append(r)
+                    if cur["rec_has_alias"][r] and len(alias):
+                        ins.append((r, r, ("rec_alias_dns", cur["rec_alias_dns"][int(rng.choice(alias))])))
+                    else:
+                        ins.append((r, r, ("values", int(rng.integers(0, n_rec)))))
+                elif c < 0.7:
+                    deleted.append(r)
+                else:
+                    ins.append((r, int(rng.integers(0, n_rec)), None))  # inserted in front of r
+            if n_rec:
+                ins.append((a, int(rng.integers(0, n_rec)), None))  # at the front (in an empty zone: its only record)
+                ins.append((b, int(rng.integers(0, n_rec)), None))  # at the end
+        if not ins:
+            continue
+        ins.sort(key=lambda x: x[0])
+        base = sum(len(p) for p in placed)
+        for k, (_, _, o) in enumerate(ins):
+            if o is not None:
+                extra[base + k] = o
+        targets.append(z)
+        placed.append([s for _, s, _ in ins])
+        at.extend(x for x, _, _ in ins)
+    if not targets:
+        return dict(rows=None, zone_target=np.zeros(0, dtype=np.uint32), rec_at=np.zeros(0, dtype=np.uint32), deleted=np.asarray(sorted(set(deleted)), dtype=np.uint32))
+    rows = actual_rows(cur)
+    rows["zone_name"] = np.asarray(cur["zone_name"], dtype=np.uint64)[np.asarray(targets, dtype=np.int64)]
+    src = [s for p in placed for s in p]
+    for k, (col, v) in extra.items():
+        if col == "values":
+            src[k] = src[k], v  # the record of src[k] with the values of record v
+    recs = [s if isinstance(s, int) else s[0] for s in src]
+    rows.update(take_tree(cur, "rec", np.asarray(recs, dtype=np.int64)))
+    vb = np.asarray(cur["rec_val_begin"]).astype(np.int64)
+    vals = [np.arange(vb[s], vb[s + 1]) if isinstance(s, int) else np.arange(vb[s[1]], vb[s[1] + 1]) for s in src]
+    rows["rec_val_begin"] = np.concatenate([[0], np.cumsum([len(v) for v in vals])]).astype(np.uint32)
+    rows["val_value"] = np.asarray(cur["val_value"])[np.concatenate(vals).astype(np.int64)] if vals else np.zeros(0, dtype=np.uint64)
+    for k, (col, v) in extra.items():
+        if col == "rec_alias_dns":
+            rows["rec_alias_dns"][k] = v
+    rows["zone_rec_begin"] = np.concatenate([[0], np.cumsum([len(p) for p in placed])]).astype(np.uint32)
+    return dict(rows=compact_actual(rows), zone_target=np.asarray(targets, dtype=np.uint32), rec_at=np.asarray(at, dtype=np.uint32),
+                deleted=np.asarray(sorted(set(deleted)), dtype=np.uint32))
+
+
+def record_refresh(resident: dict, cloud: dict, rec_rows) -> dict:
+    """The record delta that re-describes the resident record rows `rec_rows` from the cloud's tables (actual column dicts with
+    the same zone table): per row, ListResourceRecordSets(zone, StartRecordName = its name, StartRecordType = its type,
+    MaxItems = 1) — the cloud's set of that (zone, name, type) replaces the row in place, or the row is deleted when the cloud has
+    none.  The n-th resident row of a (zone, name, type) maps to the n-th cloud set of it.  -> keyword arguments of
+    Engine.apply_records / ActualMirror.apply_records."""
+    def ids(cols):
+        zb = np.asarray(cols["zone_rec_begin"]).astype(np.int64)
+        slab = np.asarray(cols["slab"]).tobytes()
+        name, typ = np.asarray(cols["rec_name"]), np.asarray(cols["rec_type"])
+        out, seen = [], {}
+        for z in range(len(zb) - 1):
+            for r in range(zb[z], zb[z + 1]):
+                o, n = int(name[r]) & ((1 << 40) - 1), int(name[r]) >> 40
+                key = (z, slab[o:o + n], int(typ[r]))
+                seen[key] = seen.get(key, -1) + 1
+                out.append(key + (seen[key],))
+        return out
+    rid, cid = ids(resident), ids(cloud)
+    where = {k: r for r, k in enumerate(cid)}
+    rows = sorted(set(int(r) for r in rec_rows))
+    zb = np.asarray(resident["zone_rec_begin"]).astype(np.int64)
+    by_zone = {}
+    for r in rows:
+        c = where.get(rid[r])
+        if c is not None:
+            by_zone.setdefault(rid[r][0], []).append((r, c))
+    zones = sorted(by_zone)
+    d = record_rows(cloud, zones, [[c for _, c in by_zone[z]] for z in zones]) if zones else None
+    return dict(rows=d, zone_target=np.asarray(zones, dtype=np.uint32), rec_at=np.asarray([r for z in zones for r, _ in by_zone[z]], dtype=np.uint32),
+                deleted=np.asarray(rows, dtype=np.uint32))
+
+
+def record_redescribe(cols: dict, rec_rows) -> dict:
+    """The record delta a worker applies after re-describing the resident record rows `rec_rows` and finding them as `cols` (the
+    mirror of the resident tables) holds them: each row replaced in place by its own set (a delete of the row plus an insert in
+    front of it).  -> keyword arguments of Engine.apply_records / ActualMirror.apply_records."""
+    rows = np.unique(np.asarray(rec_rows, dtype=np.int64).reshape(-1))
+    zb = np.asarray(cols["zone_rec_begin"]).astype(np.int64)
+    zones, counts = np.unique(np.searchsorted(zb, rows, side="right") - 1, return_counts=True)
+    d = actual_rows(cols)
+    d["zone_name"] = np.asarray(cols["zone_name"], dtype=np.uint64)[zones]
+    d.update(take_tree(cols, "rec", rows))
+    d["zone_rec_begin"] = np.concatenate([[0], np.cumsum(counts)]).astype(np.uint32)
+    return dict(rows=compact_actual(d), zone_target=zones.astype(np.uint32), rec_at=rows.astype(np.uint32), deleted=rows.astype(np.uint32))

@@ -555,6 +555,71 @@ typedef struct gar_zone_delta_result {
 } gar_zone_delta_result;
 int gar_snapshot_apply_zones(gar_engine *e, const gar_zone_delta *d, gar_zone_delta_result *out);
 
+/* ---------------------------------------------------------------- record deltas: record sets edited inside resident zones
+   Re-described record sets (ListResourceRecordSets with StartRecordName / StartRecordType / MaxItems) applied to the loaded record
+   table on the device, so that a worker refreshes the record sets its keys read (gar_read_records, below) instead of whole zone
+   record lists.  The scheme of the zone deltas, one level down.  Rules:
+     - new order, inside every zone z: for each resident record r of z in order, first the delta records with rec_at == r in delta
+       order, then r itself unless it is deleted; the delta records with rec_at == zone_rec_begin[z + 1] (behind z's last record)
+       come last.  So resident record r becomes
+         r - #{deleted rows < r} + #{k : rec_at[k] <= r},
+       and delta record k becomes
+         rec_at[k] - #{deleted rows < rec_at[k]} + k.
+       An insert behind the last record of zone z and an insert in front of the first record of zone z + 1 share the rec_at value;
+       the one of zone z comes first, which is delta order because zone_target ascends.  Replacing a record set is a delete of r
+       plus an insert at r.  Values follow their records, and zone_rec_begin and everything else are laid out exactly as a
+       gar_snapshot_load of the resulting tables would lay them out.  Load balancers, accelerators and zone rows do not move;
+     - the strings of `rows` are appended to the resident AWS slab at a 16-byte aligned slab_base, as for gar_snapshot_apply_actual;
+       slab_base is 0 when no record is inserted.
+   GAR_E_INVALID, with the snapshot unchanged: anything gar_snapshot_load rejects in an actual table; `rows` holding load
+   balancers, accelerators or any of their children; zone_target not strictly ascending or >= n_zones; a delta zone's zone_name
+   different from its resident zone's; rec_at[k] outside [zone_rec_begin[z], zone_rec_begin[z + 1]] of its zone z (the next zone's
+   interior included) or decreasing; a deleted row >= n_records or deleted twice; a NULL array with a non-zero count.  GAR_E_STATE
+   in the cases of gar_snapshot_apply_actual (before a load, on an attached snapshot, once gar_shard_route has run on the loaded
+   slice, on a sharded sub-snapshot); after a CUDA error in the middle no snapshot is loaded.  Every later gar_diff,
+   gar_diff_device, gar_diff_keys, gar_bindings_diff, gar_read_set, gar_read_records, delta, compaction and export answers bit for
+   bit as after a gar_snapshot_load of the same object table and the resulting AWS tables.  The call drops the prepared state and
+   the recorded launch sequence, as an AWS delta does. */
+typedef struct gar_record_delta {
+  const gar_actual *rows;       /* record sets with their values, grouped by delta zone (zone_rec_begin), packed like a load's actual
+                                   table with its own slab; n_lbs = n_accels = 0 and their CSRs {0}.  NULL / no records: inserts none */
+  const uint32_t *zone_target;  /* [rows->n_zones] resident zone of delta zone k; strictly ascending; zone_name equal byte for byte */
+  const uint32_t *rec_at;       /* [rows->n_records] resident record row that delta record k is listed in front of, inside
+                                   [zone_rec_begin[z], zone_rec_begin[z + 1]] of its zone z (the end = behind the zone's last record);
+                                   non-decreasing in k */
+  uint32_t n_deleted;
+  const uint32_t *deleted;      /* [n_deleted] resident record rows, removed with their values; distinct, < n_records */
+} gar_record_delta;
+typedef struct gar_record_delta_result {
+  uint32_t n_records, n_values;  /* after the delta */
+  uint64_t slab_base, slab_len;  /* as in gar_actual_delta_result */
+} gar_record_delta_result;
+int gar_snapshot_apply_records(gar_engine *e, const gar_record_delta *d, gar_record_delta_result *out);
+
+/* Record read set: the resident record rows the Route53 decisions of a keyset read, the unit of gar_snapshot_apply_records.
+   Rules (a superset of what gar_diff_keys reads, independent of which branch each decision takes):
+     - for each row i of keys->rows: every owner value of i's owned-value list (the list of the lowest row with i's key, as the
+       decisions read it; all zones): the record that carries it, and every alias record (rec_has_alias) of that zone whose name
+       equals that record's name — FindOwneredARecordSets' result plus the sets its owner-value pass walks
+       (route53.go:167-181,216-238);
+     - for each deleted key: the same, for the owner values its cleanup finds through the owner-value index.
+   Every row lies in a zone gar_read_set reports for the same keyset.
+   Guarantee: insert, delete or change any record outside the set with gar_snapshot_apply_records, and gar_diff_keys of the same
+   keyset returns the identical change set, except that the record and value rows the ops name are renumbered by the new layout.
+   Limitation: a change that decides membership — a value that becomes an owner value of a key in the set, an alias record added
+   under the name of a record in the set — is outside the set until it is listed, as for gar_read_set; the periodic full re-list
+   covers it.
+   Validation and GAR_E_STATE are gar_read_set's.  The call prepares a stale snapshot as gar_read_set does, changes nothing
+   resident and leaves the recorded launch sequence as it was.  The array is engine-owned pinned host memory, valid until
+   gar_read_records_free. */
+typedef struct gar_record_readset {
+  uint32_t n_records;
+  const uint32_t *rec_rows;  /* [n_records] ascending, distinct resident record rows */
+  void *opaque;              /* engine-private; do not touch */
+} gar_record_readset;
+int gar_read_records(gar_engine *e, const gar_keyset *keys, gar_record_readset *out);
+void gar_read_records_free(gar_engine *e, gar_record_readset *rs);
+
 /* ---------------------------------------------------------------- slab compaction: dropping the dead strings on the device
    Deltas only append to the two resident slabs.  gar_snapshot_compact rebuilds the slab of each selected group (`groups`: a
    mask of GAR_COMPACT_*) so that it holds exactly the strings the resident columns reference, entirely on the device: no byte
@@ -575,7 +640,7 @@ int gar_snapshot_apply_zones(gar_engine *e, const gar_zone_delta *d, gar_zone_de
        shared).  For a hand-packed table that interned strings slab_len may therefore grow; `out` reports it, it is no error.
      - row order, every CSR and every fixed-width column are untouched.  The slab keeps GAR_SLAB_PAD zero bytes behind slab_len.
    Every later gar_diff, gar_diff_device, gar_diff_keys, gar_bindings_diff, gar_snapshot_apply_objects,
-   gar_snapshot_apply_actual and gar_snapshot_apply_zones answers bit for bit as before the call, except that tok_name / tok_region reference the new object
+   gar_snapshot_apply_actual, gar_snapshot_apply_zones and gar_snapshot_apply_records answers bit for bit as before the call, except that tok_name / tok_region reference the new object
    slab (equal as the strings they name; gar_snapshot_read_slab resolves them) and later deltas report slab_base / slab_len
    relative to the compacted slab.
    groups == 0 or unknown bits: GAR_E_INVALID.  GAR_E_STATE in exactly the cases of gar_snapshot_apply_objects.  The new slabs and
